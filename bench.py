@@ -1,13 +1,19 @@
 #!/usr/bin/env python
-"""bench.py -- decode tokens/s (bs=1) of a Llama-2-7B-shaped EXL2 ~4.0 bpw model on the B200-native hot path,
+"""bench.py -- decode tokens/s (bs=1) of a Llama-2-7B-shaped EXL2 ~4.0 bpw model on the sm_90a (H100) hot path,
 with the q_gemm path's achieved HBM GB/s against the measured roofline.  BASELINE.json metric / configs[2].
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--model PRESET]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--model PRESET] [--dump-outputs DIR]
 
 A "step" is one decode token: embedding -> 32 x (Q4-KV unpack, RMSNorm+QKV+RoPE, paged attention, Q4-KV pack,
 O-proj+residual, RMSNorm+gate|up+silu*mul, down+residual) -> RMSNorm -> lm_head.  Weights are synthetic tensors in the
-reference's on-disk EXL2 format (no network), resident in HBM; 3.3 GB of packed weights per token >> 126 MB L2, so no
+reference's on-disk EXL2 format (no network), resident in HBM; 3.3 GB of packed weights per token >> 50 MB L2, so no
 L2 flush is needed between steps ("inputs_exceed_l2").
+
+--dump-outputs DIR writes what the last timed step returned to its caller: for decode DIR/logits.npy (float32 [1, vocab])
+and DIR/next_token.npy (float64 [1, 1], the on-device argmax fed to the next step; with --gpus N rank 0 writes the
+all-gathered logits), for --mode prefill DIR/hidden.npy (float32 [16, prompt_len, hidden], the final hidden states of the
+timed many-row pass).  Weights, prompts and synthetic cache rows are seeded, so two builds run with the same arguments
+can be compared output for output.
 
 JSON keys (one line on stdout):
   value / ms_per_step   device-timed (CUDA events) over K graph replays, next token chosen by an on-device argmax
@@ -40,6 +46,16 @@ UNIT = "tokens/s"
 # helpers
 # ---------------------------------------------------------------------------------------------------------------------
 
+def dump_outputs(outdir: str, **arrays) -> None:
+    """--dump-outputs: each array as outdir/<name>.npy, float32 (float64 for token ids)."""
+    import numpy as np
+    os.makedirs(outdir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().cpu()
+        a = a.double() if not a.is_floating_point() else a.float()
+        np.save(os.path.join(outdir, f"{name}.npy"), a.numpy())
+
+
 def measured_peaks() -> tuple[float, str]:
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -47,7 +63,7 @@ def measured_peaks() -> tuple[float, str]:
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s, not measured)"
 
 
 class ClockSampler:
@@ -285,6 +301,8 @@ def run_ours(args, rank, world):
     ms_total = e0.elapsed_time(e1)
     ms_per_step = ms_total / K
     assert bool(torch.isfinite(dec.logits).all()), "decode produced non-finite logits"
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, logits=dec.logits, next_token=dec.ids)
     value = 1000.0 / ms_per_step
 
     # ---- parity of the TIMED path: the same token through the chained launches (what the graph replays) and through the
@@ -372,19 +390,8 @@ def run_ours(args, rank, world):
     ms_gemv = e0.elapsed_time(e1) / R
     peak, peak_src = measured_peaks()
     achieved = dec.weight_bytes / (ms_gemv * 1e-3) / 1e9
-    # DRAM traffic of the kernel from the committed ncu capture (profiles/): measured bytes of one launch of a known shape;
-    # scaled by this run's algorithmic bytes per launch it says how much is re-read (ratio ~1.00: nothing)
-    traffic, traffic_note = None, "no ncu capture committed"
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_gemv_i8_traffic.json" if dec.row_gemv else "r01_gemm_tc_traffic.json")) as f:
-            tj = json.load(f)
-        ratio = tj["dram_bytes_per_launch"] / tj["algorithmic_bytes_per_launch"]
-        traffic = ratio * dec.weight_bytes / n_gemv
-        traffic_note = f"ncu dram__bytes_read+write / algorithmic = {ratio:.3f} on {tj['shape']} ({tj['source']}), applied to this run's mean launch"
-    except (OSError, KeyError, ValueError):
-        pass
     roofline = {"bound": "hbm", "kernel": "gemv_i8_kernel" if dec.row_gemv else "gemm_tc_kernel", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic, "traffic_note": traffic_note, "peak_source": peak_src, "algorithmic_bytes_per_token": dec.weight_bytes,
+                "peak_source": peak_src, "algorithmic_bytes_per_token": dec.weight_bytes,
                 "gemv_launches_per_token": n_gemv, "avg_launch_us": ms_gemv * 1e3 / n_gemv,
                 "note": f"{n_launch_roof} launches ({n_gemv} dequant-GEMMs + their prep/rope launches, if any) replayed back to back in one CUDA graph, CUDA events"}
 
@@ -441,7 +448,9 @@ def run_prefill(args):
             if i:
                 ts.append(e0.elapsed_time(e1))
         return sorted(ts)[len(ts) // 2], out
-    ms_rows, x_rows = timed(dec.prefill_rows, max(2, min(args.steps, 8)))
+    ms_rows, x_rows = timed(dec.prefill_rows, args.steps)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, hidden=x_rows)
     ms_chunk, x_chunk = timed(lambda p: dec.prefill(p, chunk=8), 1)
     # same prompt, two schedules: the hidden state of the last chunk must agree (Q4 cache in the loop: loose tolerance)
     a, b = x_rows[:, -8:].float(), x_chunk.float()
@@ -472,9 +481,15 @@ def main():
     ap.add_argument("--mode", default="decode", choices=["decode", "prefill"])
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-ref-ext", action="store_true", help="skip the reference-extension leg (oracle/_ref on the same GPU)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned as DIR/<name>.npy (decode: logits, next token; prefill: hidden states)")
     args = ap.parse_args()
-    rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes this library's outputs (--impl ours)")
+    rank = int(os.environ.get("RANK", "0"))
     if args.impl == "reference":
         return run_reference(args, rank, world)
     if args.mode == "prefill":

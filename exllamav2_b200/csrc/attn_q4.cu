@@ -39,7 +39,7 @@ struct AttnQ4Params {
     const int32_t* cache_seqlens;   // [batch]  tokens already in the cache
     const int32_t* block_table;     // [batch, pages_per_seq]
     half* out;              // [batch, q_len, H, hd]
-    half* out_xp;           // optional: the consumer matrix's (o_proj) activation buffer, UMMA layout, permuted rows
+    half* out_xp;           // optional: the consumer matrix's (o_proj) activation buffer, core-matrix layout, permuted rows
     const uint16_t* out_invperm;
     int q_len, H, KVH, hd, page_size, pages_per_seq, max_ctx;
     float scale_log2;       // softmax_scale * log2(e)
@@ -48,7 +48,7 @@ struct AttnQ4Params {
     const half* rope_sin;   // [max_pos, sincos_size] or NULL
     const half* rope_cos;
     int rope_neox, sincos_size;
-    int out_plain;          // out_xp is a plain fp16 row (single-row GEMV consumer) instead of the UMMA operand layout
+    int out_plain;          // out_xp is a plain fp16 row (single-row GEMV consumer) instead of the core-matrix operand layout
     int32_t* err;           // sticky device flag: bit 0 = a sequence ran past its page table (nothing appended, no output)
     // split-KV (long contexts, q_len == 1): grid.z CTAs share one (head, sequence); each attends a contiguous chunk of positions
     // and leaves (max, sum, unnormalised rotated output) in `ws`; the last to arrive (counter) merges.  Chunks are at least
@@ -783,9 +783,8 @@ extern "C" int exl2b_paged_attn_decode_q4_ex(const uint16_t* q, const uint16_t* 
     P.sc_len = sc_len;
     // cached rows beyond the staged window: streamed through a ring of 4 x 128 positions when the cache is long; the ring takes the
     // place of half the staged window, so the CTA keeps the footprint that lets it share an SM with one GEMV CTA (a first version
-    // that ADDED the ring lost that co-residency and 0.55 ms per token at 1 k context)
-    // Measured (decode tok/s at 1 k / 4 k / 16 k positions, ring off -> on): 469 -> 439, 355 -> 343, 153 -> 256: the ring pays once a CTA
-    // has thousands of positions; below, the larger window wins.  The host only knows the cache's capacity:
+    // that ADDED the ring lost that co-residency).  The ring pays once a CTA has thousands of positions; below, the larger window
+    // wins.  The host only knows the cache's capacity:
     P.ring_slots = (P.max_ctx > 8192) ? AQ_RING : 0;
     P.stage = P.ring_slots ? AQ_STAGE / 2 : AQ_STAGE;          // (the ring takes the place of half the window: same footprint)
     const size_t smem = (size_t)((hd / 32) * 36 + AQ_WARPS * hd + 2 * AQ_WARPS) * 4 + (size_t)(hd / 32) * (80 + 8) + 2 * AQ_MAX_QLEN * (hd / 2) + 2 * AQ_MAX_QLEN * (hd / 32) * 2 +

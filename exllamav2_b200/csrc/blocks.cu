@@ -44,7 +44,7 @@ static int chain_out(GemvExtras& ex, const exl2b_chain_t* next) {
     EXL2B_REQUIRE(next->num_consumers <= GEMV_MAX_MATS, "at most %d chained consumers", GEMV_MAX_MATS);
     for (int i = 0; i < next->num_consumers; ++i) {
         QMatrix* c = (QMatrix*)next->consumers[i];
-        EXL2B_REQUIRE(c && c->v.layout == LAYOUT_TC, "chained consumer must be a tcgen05-layout matrix");
+        EXL2B_REQUIRE(c && c->v.layout == LAYOUT_TC, "chained consumer must be a LAYOUT_TC matrix");
         int rc = qmatrix_chain_buffers(c);
         if (rc) return rc;
         ex.scat[i] = ScatterTarget{c->xp_buf, c->invperm, (const half*)next->norm_weight};
@@ -168,7 +168,7 @@ extern "C" int exl2b_qattn_forward_1_ex(exl2b_qattn_t h, const uint16_t* x, int 
                            d.num_kv_heads, past_len, past_lens, neox, d.sincos_size);
     }
     const bool fuse = gemv_supports_extras(mats, 3, rows) && (!rope || (d.head_dim <= 128 && 128 % d.head_dim == 0 && d.sincos_size <= d.head_dim));
-    EXL2B_REQUIRE(!input_prepared || fuse, "input_prepared needs the tcgen05 layout and at most %d rows", GEMV_MTOK);
+    EXL2B_REQUIRE(!input_prepared || fuse, "input_prepared needs LAYOUT_TC and at most %d rows", GEMV_MTOK);
     if (fuse) {
         GemvExtras ex = {};
         if (rope) ex.rope = RopeFuse{(const half*)sin, (const half*)cos, past_lens, past_len, q_len, d.head_dim, d.sincos_size, d.rope_style == 2, 3u};
@@ -223,7 +223,7 @@ extern "C" int exl2b_qattn_forward_2_ex(exl2b_qattn_t h, uint16_t* x, const uint
     if (!want && batch * q_len > GEMM_BIG_MIN_ROWS && gemm_big_available())
         return gemm_big_launch(mo, (const half*)attn_out, mo->v.K, (half*)x, mo->v.N, batch * q_len, a->d.has_residual ? 0 : 1, (cudaStream_t)stream);
     if (!want) return gemv_launch(a->device, (cudaStream_t)stream, &m, 1, batch * q_len, nullptr, 0.f, EPI_STORE);
-    EXL2B_REQUIRE(gemv_supports_extras(&m, 1, batch * q_len), "chained launches need the tcgen05 layout and at most %d rows", GEMV_MTOK);
+    EXL2B_REQUIRE(gemv_supports_extras(&m, 1, batch * q_len), "chained launches need LAYOUT_TC and at most %d rows", GEMV_MTOK);
     GemvExtras ex = {};
     int rc = chain_out(ex, next);
     if (rc) return rc;
@@ -334,13 +334,13 @@ extern "C" int exl2b_qmlp_forward_ex(exl2b_qmlp_t h, uint16_t* x, int rows, uint
     const int epi = d.act_gelu ? EPI_GELU_MUL : EPI_SILU_MUL;
     const bool fuse = gemv_supports_extras(gu, 2, rows) && gemv_supports_extras(&down, 1, rows);
     EXL2B_REQUIRE(fuse || (!input_prepared && !(next && next->num_consumers > 0)),
-                  "chained launches need the tcgen05 layout and at most %d rows", GEMV_MTOK);
+                  "chained launches need LAYOUT_TC and at most %d rows", GEMV_MTOK);
     if (!fuse) {
         int rc = gemv_launch(m->device, stream, gu, 2, rows, (const half*)d.layernorm, d.norm_epsilon, epi);
         if (rc) return rc;
         return gemv_launch(m->device, stream, &down, 1, rows, nullptr, 0.f, EPI_STORE);
     }
-    // gate|up writes silu(gate)*up straight into down's activation buffer (permuted, UMMA layout): no prep launch between
+    // gate|up writes silu(gate)*up straight into down's activation buffer (permuted, core-matrix layout): no prep launch between
     GemvExtras e1 = {};
     exl2b_chain_t to_down = {};
     to_down.consumers[0] = (exl2b_qmatrix_t)dn;
@@ -400,7 +400,7 @@ extern "C" int exl2b_gemm_half_q_half_prepared(exl2b_qmatrix_t h, uint16_t* c, i
     EXL2B_REQUIRE(ldc >= q->v.N, "leading dimension too small");
     EXL2B_CUDA(cudaSetDevice(q->device));
     GemvMat mt = make_mat(q, nullptr, q->v.K, (half*)c, ldc, clear ? 1 : 0);
-    EXL2B_REQUIRE(gemv_supports_extras(&mt, 1, m), "chained launches need the tcgen05 layout and at most %d rows", GEMV_MTOK);
+    EXL2B_REQUIRE(gemv_supports_extras(&mt, 1, m), "chained launches need LAYOUT_TC and at most %d rows", GEMV_MTOK);
     GemvExtras ex = {};
     const QMatrix* qc = q;
     int rc = chain_in(ex, &mt, &qc, 1, has_norm != 0);
@@ -412,7 +412,7 @@ extern "C" int exl2b_gemm_half_q_half_prepared(exl2b_qmatrix_t h, uint16_t* c, i
 extern "C" int exl2b_qmatrix_chain_target(exl2b_qmatrix_t h, uint16_t** xp, const uint16_t** invperm) {
     QMatrix* q = (QMatrix*)h;
     EXL2B_REQUIRE(q && xp && invperm, "null argument");
-    EXL2B_REQUIRE(q->v.layout == LAYOUT_TC, "chained consumer must be a tcgen05-layout matrix");
+    EXL2B_REQUIRE(q->v.layout == LAYOUT_TC, "chained consumer must be a LAYOUT_TC matrix");
     int rc = qmatrix_chain_buffers(q);
     if (rc) return rc;
     *xp = (uint16_t*)q->xp_buf;

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libexl2b200 (sm_100a only).
+// Shared host/device helpers for libexl2b200 (sm_90a).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>

@@ -139,8 +139,8 @@ EXL2B_HD void dequant_block_4bit_offset(const uint32_t* mw, uint32_t* A) {
     }
 }
 
-// Two-offset form: no shift for slots 0/1, one shift for slots 2/3 -> 4 LOP3 + 1 SHF per 8 weights, all on the ALU pipe
-// (LOP3 / SHF issue at half rate on sm_100, so the ALU pipe is what bounds the unpack; measured tools/ubench).
+// Two-offset form: no shift for slots 0/1, one shift for slots 2/3 -> 4 LOP3 + 1 SHF per 8 weights, all on the ALU pipe,
+// which is what bounds the unpack.
 //   even pair slots: (x & 0x000f000f) | 0x6400 = 1024 + q      odd pair slots: (x & 0x00f000f0) | 0x5400 = 64 + q
 // The per-slot offset (+ the zero point) is removed by one extra MMA against a constant "offset tile".
 EXL2B_HD constexpr int offset2_of_pair(int p) { return (p & 1) ? 64 : 1024; }

@@ -5,7 +5,7 @@
 namespace exl2b {
 
 constexpr int GEMV_MAX_MATS = 3;
-constexpr int GEMV_MTOK = 8;          // tokens per pass (the N=8 dimension of mma.m16n8k16)
+constexpr int GEMV_MTOK = 8;          // tokens per pass (the N=8 dimension of wgmma.m64n8k16)
 
 enum GemvEpilogue : int {
     EPI_STORE = 0,      // c = (clear ? 0 : c) + bias + acc
@@ -15,7 +15,7 @@ enum GemvEpilogue : int {
 
 struct GemvMat {
     QMatView w;
-    const half* xp;  // tcgen05 path: activations prepared by tc_prep_kernel (normalised, permuted, UMMA core-matrix layout)
+    const half* xp;  // wgmma path: activations prepared by tc_prep_kernel (normalised, permuted, core-matrix layout)
     const half* x;   // input activations fp16 [M][ldx], ORIGINAL feature order (the kernel gathers through w.perm)
     int ldx;
     half* c;         // output fp16 [M][ldc]
@@ -25,7 +25,7 @@ struct GemvMat {
     int strip_begin; // filled by the launcher
 };
 
-// ---- optional fusions around a launch (tcgen05 path) --------------------------------------------------------------------
+// ---- optional fusions around a launch (wgmma path) ----------------------------------------------------------------------
 // RoPE applied in the epilogue of the matrices selected by `mask` (cuda/rope.cu:10-123 arithmetic; needs 128 % head_dim == 0
 // so that a rotation partner lives in the same 128-column strip)
 struct RopeFuse {
@@ -36,7 +36,7 @@ struct RopeFuse {
     unsigned mask;          // bit i: rotate mat[i]'s output
 };
 // A consumer of this launch's output: its activation buffer is filled directly from the epilogue, already permuted
-// into the consumer's row order, in the UMMA core-matrix layout, times the consumer's RMSNorm weight -- the consumer
+// into the consumer's row order, in the wgmma core-matrix layout, times the consumer's RMSNorm weight -- the consumer
 // launch then needs no prep kernel.  The RMSNorm's 1/rms is deferred: the producer leaves per-strip sums of squares
 // in `sumsq`, the consumer multiplies its fp32 result by rsqrt(sum / K + eps).
 struct ScatterTarget {
@@ -71,10 +71,10 @@ struct GemvParams {
     int act_rows;          // rows staged per segment (capacity)
     unsigned long long* dbg;   // optional phase timestamps (globaltimer) of CTA dbg_cta, NULL in production
     int dbg_cta;
-    int tc_stage_bytes;    // tcgen05 kernel: bytes of one weight stage (largest group of one 32-column block)
-    int tc_act_off;        // tcgen05 kernel: shared-memory offset of the staged activations
-    int tc_act_bytes;      // tcgen05 kernel: bytes of the two activation rings
-    int tc_stages;         // tcgen05 kernel: pipeline stages (groups in flight per warp), 2..4
+    int tc_stage_bytes;    // wgmma kernel: bytes of one weight stage (largest group of one 32-column block)
+    int tc_act_off;        // wgmma kernel: shared-memory offset of the staged activations
+    int tc_act_bytes;      // wgmma kernel: bytes of the two activation rings
+    int tc_stages;         // wgmma kernel: pipeline stages (groups in flight per warp), 2..4
     int row0;              // first token row of this pass (RoPE position bookkeeping)
     GemvExtras ex;
 };
@@ -90,7 +90,7 @@ constexpr int GEMM_BIG_MIN_ROWS = 16;
 bool gemm_big_available();
 int gemm_big_launch(const QMatrix* q, const half* a, int lda, half* c, int ldc, int M, int clear, cudaStream_t stream);
 
-// can `ex` be honoured for these matrices / this row count?  (tcgen05 layout, one pass)
+// can `ex` be honoured for these matrices / this row count?  (LAYOUT_TC, one pass)
 bool gemv_supports_extras(const GemvMat* mats, int nm, int M);
 
 }  // namespace exl2b

@@ -3,9 +3,9 @@
 // 140-565, q_gemm_kernel_gptq.cuh:60-225) together with the kernels the reference runs in front of them (rms_norm_kernel,
 // cuda/rms_norm.cu:55-143; act_mul_kernel, cuda/q_mlp_activation.cuh:54-100), which here are the kernel's PROLOGUE.
 //
-// Why integers: measured on B200 (tools/ubench/dp4a.cu, profiles/r02_ubench_dp4a_pdlchain.txt) the reference's recipe
-// (unpack to fp16, HFMA2) tops out at 38-44 4-bit weights/clk/SM while HBM delivers 45; the same loop on the integer
-// dot-product instruction (IDP.4A) runs at 75-98.  So the row is quantised ONCE per launch to 16-bit integers per 128-k
+// Why integers: the reference's recipe (unpack to fp16, HFMA2) spends several CUDA-core instructions per weight, while the
+// integer dot-product instruction (IDP.4A) consumes four packed fields per instruction (tools/ubench/dp4a.cu measures both
+// loops on the GPU at hand).  So the row is quantised ONCE per launch to 16-bit integers per 128-k
 // block with a power-of-two scale (signed high byte plane + unsigned low byte plane; values within 16x of the block
 // maximum are exact, the rest carry |error| <= 2^-15 of the block maximum), packed weight fields are fed to dp4a without
 // being expanded ((w & 0x0f0f0f0f) and (w & 0xf0f0f0f0) ARE four byte operands), integer sums are exact, and one fp32
@@ -16,7 +16,7 @@
 //   * one CTA per SM, 16 warps, <= 111 KB of shared memory: TWO consecutive launches are co-resident.  A CTA's first action is
 //     griddepcontrol.launch_dependents and every warp requests its first weight stages BEFORE griddepcontrol.wait, so while
 //     launch N computes, launch N+1 is already filling its arenas and HBM keeps streaming across the kernel boundary
-//     (5.1 TB/s for a decode-shaped chain of dependent launches vs 3.9 TB/s in plain stream order, tools/ubench/pdlchain.cu).
+//     (tools/ubench/pdlchain.cu compares a decode-shaped chain of dependent launches with and without this overlap).
 //   * every grid is EXACTLY one CTA per SM: CTAs without blocks are slot holders (see the kernel), so no SM ever runs two CTAs
 //     of the same launch while another idles.
 //   * a CTA owns WHOLE 32-column blocks (all of K), its 16 warps split the blocks' K range between them: split-K never leaves
@@ -28,7 +28,6 @@
 //     main loop; per quantisation group one fp32 FMA with a scale read from the matrix' dense scale table (QMatrix::wtab).
 //   * when the producer of the row scattered a copy in this matrix's stored-row order (I8Out::c_perm), the prologue reads the
 //     row with one 16-byte load per thread instead of eight 2-byte gathers.
-// Measured history of these choices: profiles/r02_history.md.
 #include <string.h>
 
 #include <algorithm>
@@ -119,7 +118,7 @@ __device__ __forceinline__ int dp4a_uu(uint32_t a, uint32_t b, int c) {
 }
 
 // descriptor / scale loads with L1 policies: the (small, re-read) stage lists are kept, the (read-once) scale entries pass through.
-// With 222 KB of the SM's 256 KB configured as shared memory the L1 is 28 KB for 32 warps; measured global-load hit rate 40%.
+// With 222 KB of the SM's 256 KB configured as shared memory the L1 is 28 KB for 32 warps.
 __device__ __forceinline__ uint4 ldg_keep(const uint4* p) {
     uint4 v;
     asm volatile("ld.global.nc.L1::evict_last.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
@@ -348,8 +347,7 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
 
     // ---- slot holders.  The grid always has one CTA per SM.  With two launches co-resident per SM, every SM must host exactly
     //      ONE CTA of every launch of the chain: an SM that has none would offer two free slots to the next launch, which then
-    //      runs two of its CTAs there at half speed each while another SM idles (measured: 10-17 SMs per launch, +50% on the
-    //      launch).  So CTAs without blocks stay resident until the CTAs with blocks are done, then leave with them.
+    //      runs two of its CTAs there at half speed each while another SM idles.  So CTAs without blocks stay resident until the CTAs with blocks are done, then leave with them.
     if ((int)blockIdx.x >= P.busy_ctas) {
         if (tid == 0) {
             while (*reinterpret_cast<volatile unsigned int*>(P.slot_cnt) < (unsigned)P.busy_ctas) __nanosleep(200);
@@ -426,8 +424,8 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
     issue_stages(0, n_pre, load_req(0));
     int next_req = n_pre;
     // EXPERIMENT, off by default (EXL2B_I8_L2PF=1): pull the rest of the warp's share into L2 now (one bulk prefetch per stage),
-    // while the previous launch is still computing.  Measured on B200 it LOSES 6% of the decode step (530 -> 496 tok/s): the
-    // 20-30 MB burst of the next launch competes with the running launch's own refills (profiles/r02_history.md)
+    // while the previous launch is still computing.  Off because the 20-30 MB burst of the next launch competes with the
+    // running launch's own refills.
     if (P.l2_prefetch)
         for (int s0 = n_pre; s0 < nst; s0 += 32) {
             const int s = s0 + lane;
@@ -1002,7 +1000,7 @@ int gemv_i8_launch(int device, cudaStream_t stream, const I8Out* outs, int nm, c
         const QMatrix* q = outs[i].q;
         EXL2B_REQUIRE(q && outs[i].c, "null matrix / output");
         const QMatView& v = q->v;
-        EXL2B_REQUIRE(v.layout == LAYOUT_TC, "matrix is not in the tcgen05 layout");
+        EXL2B_REQUIRE(v.layout == LAYOUT_TC, "matrix is not in the default (LAYOUT_TC) layout");
         EXL2B_REQUIRE(v.KS == P.KS, "fused matrices must share K");
         EXL2B_REQUIRE((v.perm == nullptr) == (P.perm == nullptr), "fused matrices must share their row permutation");
         EXL2B_REQUIRE(q->wtab, "matrix has no scale table");

@@ -33,9 +33,9 @@ struct I8Out {
 
 // One launch over `nm` matrices that share K, the input row and the row permutation.  M = 1 only.
 int gemv_i8_launch(int device, cudaStream_t stream, const I8Out* outs, int nm, const I8Input& in);
-// same K / same permutation contents / tcgen05 layout?  (host check, synchronises once; call at block-creation time)
+// same K / same permutation contents / LAYOUT_TC?  (host check, synchronises once; call at block-creation time)
 bool gemv_i8_fusable(const QMatrix* const* qs, int nm);
-// EXL2B_GEMV=tc in the environment routes single rows through the tcgen05 kernel instead (A/B comparisons)
+// EXL2B_GEMV=tc in the environment routes single rows through the wgmma kernel (gemm_tc.cu) instead (A/B comparisons)
 bool gemv_i8_enabled();
 
 }  // namespace exl2b

@@ -3,7 +3,7 @@
 //
 // The reference keeps the checkpoint's [packed-row, column] order and re-shuffles bit fields inside each 32-row column unit at
 // load time (exllamav2_ext/cuda/q_matrix.cu:21-44, quant/qdq_*.cuh shuffle_*).  We do a different load-time re-pack (same
-// total bytes, written back over q_weight exactly like the reference mutates it) into a layout built for B200 streaming.
+// total bytes, written back over q_weight exactly like the reference mutates it) into a layout built for streaming with TMA bulk copies.
 //
 // THE layout every kernel uses (LAYOUT_TC below):
 //   strip  = 128 output columns = 4 blocks; block = 32 k x 32 n; every block's slabs (32 stored rows k' each) form their own
@@ -12,8 +12,8 @@
 //   lane l of a block owns column n = l and all 32 k of the slab: value i <-> k_local = i, pair p = i / 2 = (k, k+1).
 //   plane  = a b-bit value is split into power-of-two bit planes (b = main + extra: 2=2, 3=2+1, 4=4, 5=4+1, 6=4+2, 8=8) with
 //            field e of pair slot j at bit 16e + P*j of its word, so that
-//              * `(w >> sh) & mask | magic` is a valid fp16 pair (the 0x6400 trick generalised to every exponent): the tcgen05
-//                kernel writes it straight to tensor memory as one 32-bit TMEM column of row n (gemm_tc.cu);
+//              * `(w >> sh) & mask | magic` is a valid fp16 pair (the 0x6400 trick generalised to every exponent): the wgmma
+//                kernel stores it straight into row n of its shared-memory A tile (gemm_tc.cu);
 //              * `w & 0x0f0f0f0f` / `w & 0xf0f0f0f0` (and the 2- / 1-bit analogues) are four BYTE operands of the integer
 //                dot-product instruction: the batch-1 GEMV feeds packed words to dp4a unexpanded (gemv_i8.cu).
 //
@@ -121,13 +121,13 @@ EXL2B_HD constexpr int index_of(int n_local, int k_local) {
     return p * 2 + e;
 }
 
-// ---- second lane mapping ("TC" layout, used by the tcgen05 kernel) ----------------------------------------------------
+// ---- second lane mapping ("TC" layout, used by the wgmma kernel) ------------------------------------------------------
 // strip = 128 columns = 4 blocks; each block's slabs form their own contiguous stream ([strip][blk][slab]), lane l of a
 // block owns column n = l and all 32 k of the slab: value i <-> k_local = i, pair p = i/2 = (k, k+1).  After unpacking,
-// register p of lane l is half2(W[k=2p][n], W[2p+1][n]) -- exactly one 32-bit TMEM column of row n of the UMMA A
-// operand (M = 128 weight columns on the TMEM lanes, K along TMEM columns), written with tcgen05.st.32x32b.
+// register p of lane l is half2(W[k=2p][n], W[2p+1][n]) -- four registers are one 16-byte core-matrix row (8 k) of row n of
+// the wgmma A operand (M = 128 weight columns, no-swizzle K-major tile in shared memory).
 constexpr int LAYOUT_MMA = 0;   // mma.sync fragment layout above (strip 64)
-constexpr int LAYOUT_TC = 1;    // tcgen05 / TMEM row layout (strip 128)
+constexpr int LAYOUT_TC = 1;    // column-per-lane row layout (strip 128)
 EXL2B_HD constexpr int strip_n(int layout) { return layout == LAYOUT_TC ? 128 : 64; }
 EXL2B_HD constexpr int strip_blocks(int layout) { return layout == LAYOUT_TC ? 4 : 2; }
 EXL2B_HD constexpr ValuePos value_pos_l(int layout, int lane, int i) {

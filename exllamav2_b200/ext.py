@@ -22,7 +22,7 @@ _LIB_PATH = os.path.join(_HERE, "libexl2b200.so")
 
 if not os.path.exists(_LIB_PATH):
     raise ImportError(
-        f"{_LIB_PATH} is missing: build it with `python -m exllamav2_b200.build` (nvcc, sm_100a). "
+        f"{_LIB_PATH} is missing: build it with `python -m exllamav2_b200.build` (nvcc, sm_90a). "
         "exllamav2_b200 has no CPU fallback.")
 
 lib = ctypes.CDLL(_LIB_PATH)

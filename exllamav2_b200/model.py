@@ -244,7 +244,7 @@ class ExLlamaV2Decoder:
         # True: attention reads the Q4 cache directly (one kernel per layer); False: the reference's sequence
         # q_to_fp16_kv -> attention on the fp16 temp -> fp16_to_q_kv (three kernels + the temp round trip)
         self.fused_attn = os.environ.get("EXL2B_REF_KV_SEQUENCE") is None
-        # producer epilogues feed consumer activation buffers (needs the default tcgen05 matrix layout)
+        # producer epilogues feed consumer activation buffers (needs the default LAYOUT_TC matrix layout)
         self.chained = os.environ.get("EXL2B_NO_CHAIN") is None
         # single rows (bs = 1 decode) run on the HBM-bound integer GEMV (csrc/gemv_i8.cu) in the reference's own op sequence
         self.row_gemv = os.environ.get("EXL2B_GEMV", "")[:1] != "t"

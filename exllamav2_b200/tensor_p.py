@@ -332,6 +332,8 @@ def run_bench(args, rank: int, world: int, metric: str, unit: str):
     dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms_per_step = float(ms.item()) / K
     finite = bool(torch.isfinite(dec.logits).all())
+    if args.dump_outputs and rank == 0:          # the logits are all-gathered: rank 0 holds the whole row
+        bench_mod.dump_outputs(args.dump_outputs, logits=dec.logits, next_token=dec.ids)
 
     # e2e: host token in, host logits out, every step (rank 0's host feeds all ranks through a broadcast of the id)
     ids_host = torch.zeros((1, 1), dtype=torch.long).pin_memory()
@@ -373,13 +375,13 @@ def run_bench(args, rank: int, world: int, metric: str, unit: str):
             "e2e": {"value": 1.0 / t_e2e, "unit": unit, "h2d_bytes_per_step": 8, "d2h_bytes_per_step": cfg.vocab_size * 2, "ms_per_step": t_e2e * 1e3},
             "gpu_launches": int(launches_per_step * K * world), "launches_per_step": int(launches_per_step),
             "roofline": {"bound": "hbm", "kernel": "gemv_i8_kernel", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": None, "peak_source": peak_src,
+                         "peak_source": peak_src,
                          "note": "per-GPU algorithmic weight bytes / whole step time (collectives and attention included): a lower bound on the kernel's own rate"},
             "cpu_baseline": None,
         }
         print(json.dumps(line), flush=True)
     # Leave without tearing NCCL down: destroying a communicator that live CUDA graphs still reference blocks forever
-    # (seen on 2 x B200, torch 2.11 / NCCL 2.28); the process is at its end anyway.
+    # (seen with torch 2.11 / NCCL 2.28); the process is at its end anyway.
     torch.cuda.synchronize()
     dist.barrier()
     import sys

@@ -1,4 +1,4 @@
-/* exl2_b200.h -- C ABI of libexl2b200.so: the B200-native (sm_100a) quantized-linear hot path of ExLlamaV2.
+/* exl2_b200.h -- C ABI of libexl2b200.so: the H100 (sm_90a) quantized-linear hot path of ExLlamaV2.
  *
  * Drop-in boundary (SURVEY.md 8b): the reference binds this path through the pybind11 module `exllamav2_ext`
  * (exllamav2/exllamav2_ext/ext_bindings.cpp:27-138).  Every entry point below names the reference binding it
@@ -215,7 +215,7 @@ int exl2b_paged_attn_clear_status(int device);
  * activation buffer of the matrices that consume it -- permuted through their q_invperm, in the tensor-core operand
  * layout, pre-multiplied by the RMSNorm weight they apply -- together with per-strip sums of squares; the consumer
  * launch (`input_prepared` = 1) then starts without a prep kernel and applies 1/rms to its fp32 result.
- * Valid for rows <= 8 (decode) and the default (tcgen05) matrix layout; the calls fail otherwise.
+ * Valid for rows <= 8 (decode) and the default (LAYOUT_TC) matrix layout; the calls fail otherwise.
  * `out_consumer` of exl2b_paged_attn_decode_q4 is the same mechanism for the attention output (o_proj). */
 typedef struct {
     exl2b_qmatrix_t consumers[3];   /* matrices whose INPUT is this launch's output (e.g. the next block's q, k, v) */

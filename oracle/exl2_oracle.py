@@ -5,10 +5,10 @@ __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs use 
 
 Parity status: PINNED against the reference extension itself.  The reference holds no golden vectors for this
 path (SURVEY.md 8c), so `oracle/gen_golden.py` runs the unmodified reference CUDA extension (built by
-oracle/build_ref.py into oracle/_ref/) on a B200 over the seeded tensors from `oracle/synth.py` and stores its
+oracle/build_ref.py into oracle/_ref/) on a GPU over the seeded tensors from `oracle/synth.py` and stores its
 outputs under tests/golden/; tests/test_oracle_golden.py checks every function below against them.
 
-All citations are path:line relative to /root/reference/exllamav2/ .
+All citations are path:line relative to exllamav2/ in the reference checkout.
 
 Formats (SURVEY.md Appendix B):
   EXL2  q_weight int32[R,N]  bit-strips in descending bit width; within a strip each column is a little-endian

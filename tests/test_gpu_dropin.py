@@ -1,5 +1,5 @@
 """The drop-in, EXECUTED: the reference's own Python modules (exllamav2/linear.py, rmsnorm.py, ext.py -- byte-compiled from
-/root/reference into oracle/_ref/pypkg by oracle/build_ref.py, because /root/reference does not exist on the GPU box) run
+the reference checkout into oracle/_ref/pypkg by oracle/build_ref.py, so that the GPU machine needs no checkout) run
 on top of exllamav2_b200.ext installed under the name the reference imports (`exllamav2_ext`, exllamav2/ext.py:106-109).
 
   * ExLlamaV2Linear.load(dict) -> ext.make_q_matrix (ext.py:325-410) -> our make_q_matrix, EXL2 and GPTQ (+ act-order);
@@ -8,7 +8,8 @@ on top of exllamav2_b200.ext installed under the name the reference imports (`ex
   * ExLlamaV2RMSNorm.forward -> ext_c.rms_norm (rmsnorm.py:141);
   * names outside the hot path reach the registered stock extension through the module-level forwarder, or raise an
     AttributeError that says so.
-Skipped when oracle/_ref/pypkg has not been built (python oracle/build_ref.py).
+The first two skip when oracle/_ref/pypkg has not been built (python oracle/build_ref.py); the forwarder test registers a
+stand-in stock module when the reference extension is not built.
 """
 import os
 import sys
@@ -97,16 +98,34 @@ def test_reference_rmsnorm_on_dropin(ref_py):
     assert np.abs(key(y.cpu().numpy()) - key(want)).max() <= 1
 
 
-def test_out_of_scope_names_forward_to_stock(ref_py):
-    b = ref_py.b200
+def _stand_in_stock():
+    """A module exporting two of the stock extension's out-of-scope names with its semantics: tensor_remap permutes the
+    columns of a 2-D int32 tensor in place (ext_stloader.cpp:159-219), sample_basic is only looked up."""
+    m = types.ModuleType("exllamav2_ext_stock")
+
+    def tensor_remap(t, idx):
+        t.copy_(t[:, idx.long()])
+
+    def sample_basic(*args):
+        raise NotImplementedError
+
+    m.tensor_remap, m.sample_basic = tensor_remap, sample_basic
+    return m
+
+
+def test_out_of_scope_names_forward_to_stock():
+    """Names outside the hot path reach the registered stock extension through the module-level forwarder (the reference's
+    own build when oracle/_ref has it, else a stand-in module), or raise an AttributeError that says so."""
+    import exllamav2_b200.ext as b
+    b.install_as_exllamav2_ext()
+    import exllamav2_ext                               # the name the reference's exllamav2/ext.py imports
+    assert exllamav2_ext is b
     b.set_stock_extension(None)
     with pytest.raises(AttributeError, match="outside the quantized-linear hot path"):
         b.sample_basic
     sys.path.insert(0, os.path.join(ROOT, "oracle"))
     from build_ref import load_ref
-    stock = load_ref()
-    if stock is None:
-        pytest.skip("oracle/_ref extension not built")
+    stock = load_ref() or _stand_in_stock()
     b.set_stock_extension(stock)
     try:
         assert b.sample_basic is stock.sample_basic            # exllamav2/generator/sampler.py calls ext_c.sample_basic
@@ -114,7 +133,7 @@ def test_out_of_scope_names_forward_to_stock(ref_py):
         t = torch.arange(8 * 4, dtype=torch.int32).view(8, 4).contiguous()
         idx = torch.tensor([3, 2, 1, 0], dtype=torch.int32)
         want = t[:, idx.long()].clone()
-        ref_py.ext.ext_c.tensor_remap(t, idx)
+        exllamav2_ext.tensor_remap(t, idx)
         assert torch.equal(t, want)
     finally:
         b.set_stock_extension(None)

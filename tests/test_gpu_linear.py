@@ -228,7 +228,7 @@ def test_prefill_2048_rows_llama_shape():
 
 def test_two_streams_do_not_share_scratch():
     """Calls on different streams of one device run concurrently and must not share scratch (SURVEY.md 8b: re-entrant per handle):
-    every row regime (1 row: integer GEMV, 4 rows: tcgen05 kernel, 40 rows: dense path), two matrices, two streams, many
+    every row regime (1 row: integer GEMV, 4 rows: wgmma kernel, 40 rows: dense path), two matrices, two streams, many
     interleaved launches; results must equal the serial ones bit for bit."""
     from exllamav2_b200 import ext as ext_c
     lin_a, _ = _load("b54_g64")

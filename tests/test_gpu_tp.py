@@ -1,4 +1,4 @@
-"""Column-sharded decode on 2 GPUs == single-GPU decode (tools/tp_check.py under torchrun).  Skipped on a 1-GPU box;
+"""Column-sharded decode on 2 GPUs == single-GPU decode (tools/tp_check.py under torchrun).  Skipped with a single GPU;
 the host-side logic is covered on CPU by tests/test_tp_gloo.py."""
 import os
 import subprocess

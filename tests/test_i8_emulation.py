@@ -1,7 +1,7 @@
 """CPU emulation of the index / byte-order logic of csrc/gemv_i8.cu (no GPU): the parts of the batch-1 integer GEMV
 that are pure bookkeeping and that a wrong constant would break silently.
 
-1. consume_slab: for every bit width, compose a 32 k x 32 column block in the tcgen05 layout (layout.h
+1. consume_slab: for every bit width, compose a 32 k x 32 column block in the TC layout (layout.h
    compose_lane_words), stage a row of 16-bit integers in the order stage_round writes it (high / low byte planes,
    bytes of octet j ordered k = 8j + {0,4,1,5} | {2,6,3,7}) and run the kernel's mask / shift sequence (no operand is permuted:
    layout.h pair_word / pair_slot give every plane the same byte order); the

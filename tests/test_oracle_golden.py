@@ -1,4 +1,4 @@
-"""Pin the CPU oracle against golden vectors produced by the UNMODIFIED reference CUDA extension on a B200
+"""Pin the CPU oracle against golden vectors produced by the UNMODIFIED reference CUDA extension
 (oracle/gen_golden.py -> tests/golden/*.npz).  Runs without a GPU."""
 import glob
 import os

@@ -128,8 +128,7 @@ def main():
                         r = st[i]
                         print(json.dumps({"shape": name, "M": M, "cta": cta, "launch": i, "grid_start": r[6] - t0, "grid_end": r[7] - t0,
                                           "rel_to_grid_start[start,requested,wait_done,staged,warp0_done,all_warps_done]": [x - r[6] for x in r[:6]], "grid_ns": r[7] - r[6],
-                                          "cta[start,prefetched,wait_done,staged,consumed,done]": [x - t0 for x in r[:6]],
-                                          "clk[w0|w1|w4: waits(weights+A_free),unpack,drain:wait_D,drain:rest ; w8(issue): waits(act+A_full),S+arrive,MMAs,commits]": [r[8:12], r[12:16], r[16:20], r[20:24]]}), flush=True)
+                                          "cta[start,prefetched,wait_done,staged,consumed,done]": [x - t0 for x in r[:6]]}), flush=True)
             t_eager = time_loop(run_new, 5)
             # graph-captured cycle (no host launch overhead)
             g = torch.cuda.CUDAGraph()

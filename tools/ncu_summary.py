@@ -40,5 +40,5 @@ if len(src) > 2:
     print(f"\n## SASS mix ({tot} warp instructions, {totS} stall samples)\n\n| opcode | executed | share | stall samples |\n|---|---|---|---|")
     for o, c in op.most_common(18):
         print(f"| {o} | {c} | {100*c/tot:.1f}% | {100*ops[o]/totS:.1f}% |")
-    present = [k for k in ("UTCHMMA", "STTM", "LDTM", "UBLKCP", "SYNCS", "UTCBAR") if any(k in r[iS] for r in data)]
-    print(f"\ntcgen05 / TMA mnemonics present in the SASS: {', '.join(present)}")
+    present = [k for k in ("HGMMA", "UBLKCP", "SYNCS", "WARPSYNC") if any(k in r[iS] for r in data)]
+    print(f"\nwgmma / TMA mnemonics present in the SASS: {', '.join(present)}")

@@ -1,6 +1,6 @@
 // How fast can an SM pull HBM through per-warp cp.async.bulk rings?  Same fetch pattern as gemm_tc_kernel (every warp
 // streams its own contiguous region in `stage` byte copies, `stages` in flight), but the consumer only waits and re-arms.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o bulkfetch bulkfetch.cu && ./bulkfetch
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o bulkfetch bulkfetch.cu && ./bulkfetch
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>

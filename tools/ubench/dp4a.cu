@@ -5,7 +5,7 @@
 //      activations split into a signed high and an unsigned low byte plane), weights as LDS.128 (TC layout: one column per
 //      lane, 8 k per word), activations as broadcast LDS.128.  Reports 4-bit weights / clk / SM; HBM needs 45 at 6.5 TB/s.
 //   C: the reference-style HFMA2 loop (4 LOP3 + 1 SHF + 4 HADD2/HFMA2 + 4 HFMA2 per 8 weights) for comparison.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o dp4a dp4a.cu && ./dp4a
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o dp4a dp4a.cu && ./dp4a
 #include <cstdio>
 #include <cstdint>
 #include <cuda_fp16.h>

@@ -1,6 +1,6 @@
 // Cost of a grid-wide phase barrier for a persistent decode kernel (DESIGN.md 7.1): 296 co-resident CTAs x 320 threads,
 // one arrival per CTA on a global counter, everyone spins until all have arrived.  NOT YET RUN (written after round 1's
-// GPU budget was spent).   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gridbar gridbar.cu && ./gridbar
+// GPU budget was spent).   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o gridbar gridbar.cu && ./gridbar
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

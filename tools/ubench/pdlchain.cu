@@ -4,7 +4,7 @@
 // next kernel's CTAs become resident early and fill their rings BEFORE griddepcontrol.wait, so HBM keeps streaming across
 // the kernel boundary.  Reports us / launch and TB/s for: plain stream order, PDL, PDL with a full-SM footprint (no
 // co-residency), and a decode-shaped sequence (Q|K|V 25.5 MB, attention stub, O 8.5, gate|up 45.6, down 22.8) x 32.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pdlchain pdlchain.cu && ./pdlchain
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pdlchain pdlchain.cu && ./pdlchain
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>

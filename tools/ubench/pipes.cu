@@ -1,5 +1,5 @@
-// Pipe-throughput calibration on B200: legacy mma.sync (HMMA.16816.F32), LOP3, HADD2, LDS.128.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pipes pipes.cu && ./pipes
+// Pipe-throughput calibration: legacy mma.sync (HMMA.16816.F32), LOP3, HADD2, LDS.128.
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pipes pipes.cu && ./pipes
 #include <cstdio>
 #include <cstdint>
 #include <cuda_fp16.h>
