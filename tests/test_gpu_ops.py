@@ -74,6 +74,30 @@ def test_rope(neox, batch, q_len, heads, hd):
     assert np.array_equal(cases.u16(xt2.cpu().numpy()), cases.u16(want2))
 
 
+@pytest.mark.parametrize("neox", [True, False])
+@pytest.mark.parametrize("hd", [64, 128])
+def test_rope_partial_rotary(neox, hd):
+    """sincos_size = head_dim / 2 (partial rotary): the first sincos_size dimensions of every head rotate, the rest pass
+    through untouched; bit-exact against the oracle with its rotary width, per-sequence offsets and past_len = -1."""
+    from exllamav2_b200 import ext as ext_c
+    batch, q_len, heads, rot = 3, 4, 4, hd // 2
+    rng = np.random.default_rng(hd + neox)
+    sin, cos = oracle.rope_tables(rot, 64)
+    x = rng.normal(0, 1, size=(batch, q_len, heads * hd)).astype(np.float16)
+    fn = oracle.rope_neox if neox else oracle.rope_gptj
+    st, ct = torch.from_numpy(sin).to(DEV), torch.from_numpy(cos).to(DEV)
+    for past_len, offs in ((5, np.array([0, 7, 2], dtype=np.int32)), (-1, np.array([11, 0, 3], dtype=np.int32))):
+        xt = torch.from_numpy(x).to(DEV)
+        ext_c.rope_(xt, st, ct, past_len, heads, hd, torch.from_numpy(offs).to(DEV), neox)
+        base = offs if past_len == -1 else past_len + offs
+        want = np.stack([fn(x[b].reshape(q_len, heads, hd), sin, cos, base[b] + np.arange(q_len), rot).reshape(q_len, heads * hd)
+                         for b in range(batch)])
+        got = xt.cpu().numpy()
+        assert np.array_equal(cases.u16(got), cases.u16(want)), f"past_len {past_len}"
+        assert np.array_equal(cases.u16(got.reshape(batch, q_len, heads, hd)[..., rot:]),
+                              cases.u16(x.reshape(batch, q_len, heads, hd)[..., rot:]))
+
+
 def test_act_mul():
     from exllamav2_b200 import ext as ext_c
     rng = np.random.default_rng(3)
@@ -85,6 +109,24 @@ def test_act_mul():
     got = gt.float().cpu().numpy()
     # hexp / hrcp are approximate intrinsics (q_mlp_activation.cuh:13-22): a few fp16 ulp
     assert np.allclose(got, want, rtol=4e-3, atol=2e-3)
+
+
+def test_act_mul_gelu():
+    """act_gelu: tanh-form GELU in fp32 (tanh.approx on the GPU), rounded to fp16, times up in fp16 -- a few fp16 ulp from the
+    exact-tanh oracle.  The gate spans the tanh saturation on both sides and the cubic term's range."""
+    from exllamav2_b200 import ext as ext_c
+    rng = np.random.default_rng(4)
+    g = rng.normal(0, 2, size=(5, 11008)).astype(np.float16)
+    g[0, :64] = np.linspace(-12, 12, 64).astype(np.float16)
+    u = rng.normal(0, 1, size=(5, 11008)).astype(np.float16)
+    gt = torch.from_numpy(g).to(DEV)
+    ext_c.act_mul(gt, torch.from_numpy(u).to(DEV), act_gelu=True)
+    want = oracle.gelu_mul(g, u)
+    got = gt.cpu().numpy()
+    # (tanh.approx has ~2^-11 relative error; where tanh(t) -> -1 the 1 + tanh cancellation turns that into an absolute error)
+    assert np.allclose(got.astype(np.float32), want.astype(np.float32), rtol=4e-3, atol=2e-3)
+    # not silu: the two activations differ by far more than the tolerance on this range
+    assert not np.allclose(got.astype(np.float32), oracle.silu_mul(g, u).astype(np.float32), rtol=4e-3, atol=2e-3)
 
 
 @pytest.mark.parametrize("shape", [(2, 16, 32, 128), (1, 8, 4, 64), (3, 4, 8, 128)])
@@ -241,12 +283,12 @@ def test_paged_attn_decode_q4(H, KVH, hd, q_len, seqlens):
 
 def _lin(w_np, K, N):
     from exllamav2_b200.linear import ExLlamaV2Linear, load_tensor_dict
-    lin = ExLlamaV2Linear(K, N, device=DEV)
+    lin = ExLlamaV2Linear(K, N, has_bias="bias" in w_np, device=DEV)
     lin.load(load_tensor_dict(w_np, DEV))
     return lin
 
 
-@pytest.mark.parametrize("rows", [1, 3, 8, 11])
+@pytest.mark.parametrize("rows", [1, 3, 8, 9, 11])
 @pytest.mark.parametrize("gptq", [False, True])
 def test_q_attn_block(rows, gptq):
     from exllamav2_b200 import ext as ext_c
@@ -292,14 +334,18 @@ def test_q_attn_block(rows, gptq):
     for l in (lq, lk, lv, lo): l.unload()
 
 
-@pytest.mark.parametrize("rows", [1, 2, 8, 13])
-def test_q_mlp_block(rows):
+def _q_mlp_block(rows, act_gelu, bias, share_perm=False):
+    """rows 1: integer GEMV with act*mul as the down launch's prologue when gate and up share their row permutation (as converted
+    checkpoints do), otherwise the one-row wgmma pass; 2..8: one wgmma pass with the paired gate|up
+    epilogue; 9..16: two passes (9: an 8-row pass and a one-row tail pass); > 16: dense GEMMs + act_mul."""
     from exllamav2_b200 import ext as ext_c
     from exllamav2_b200.ext import none_tensor
     hidden, inter = 256, 704       # 704 = 11 strips of 64
-    wg = synth.make_exl2(hidden, inter, (4, 3), (0.1, 0.9), 128, seed=5, scale_max_range=(0.02, 0.08))
-    wu = synth.make_exl2(hidden, inter, (4,), (1.0,), 32, seed=6, scale_max_range=(0.02, 0.08))
+    wg = synth.make_exl2(hidden, inter, (4, 3), (0.1, 0.9), 128, seed=5, scale_max_range=(0.02, 0.08), bias=bias)
+    wu = synth.make_exl2(hidden, inter, (4,), (1.0,), 32, seed=6, scale_max_range=(0.02, 0.08), bias=bias)
     wd = synth.make_exl2(inter, hidden, (6, 5), (0.1, 0.9), 32, seed=7, scale_max_range=(0.02, 0.08))
+    if share_perm:
+        wu["q_invperm"] = wg["q_invperm"].copy()
     Wg, Wu, Wd = oracle.exl2_reconstruct(wg), oracle.exl2_reconstruct(wu), oracle.exl2_reconstruct(wd)
     lg, lu, ld = _lin(wg, hidden, inter), _lin(wu, hidden, inter), _lin(wd, inter, hidden)
     rng = np.random.default_rng(rows + 50)
@@ -309,15 +355,37 @@ def test_q_mlp_block(rows):
     tb = torch.empty_like(ta)
     nw = torch.from_numpy(norm_w).to(DEV)          # must outlive the handle (raw pointer, like the reference)
     h = ext_c.make_q_mlp(nw, none_tensor, True, 1e-5, lg.q_handle, lu.q_handle, ld.q_handle,
-                         none_tensor, ta, tb, none_tensor, 64, False, True, none_tensor, none_tensor, False, True)
+                         none_tensor, ta, tb, none_tensor, 64, act_gelu, True, none_tensor, none_tensor, False, True)
     xt = torch.from_numpy(x).to(DEV)
     ext_c.q_mlp_forward_(h, xt)
     xn = oracle.rms_norm(x, norm_w, 1e-5)
-    g = oracle.gemm_truth(xn, Wg).astype(np.float16)
-    u = oracle.gemm_truth(xn, Wu).astype(np.float16)
-    a = oracle.silu_mul(g, u)
-    assert oracle.rel_l2(ta.cpu().numpy(), a) <= 3e-3          # intermediate silu(gate)*up (approximate hexp/hrcp)
+    g = oracle.gemm_truth(xn, Wg, wg.get("bias")).astype(np.float16)
+    u = oracle.gemm_truth(xn, Wu, wu.get("bias")).astype(np.float16)
+    a = (oracle.gelu_mul if act_gelu else oracle.silu_mul)(g, u)
+    # intermediate act(gate)*up (approximate hexp/hrcp, tanh.approx); the single-row path never materialises it
+    if rows > 1:
+        assert oracle.rel_l2(ta.cpu().numpy(), a) <= 3e-3
+        other = (oracle.silu_mul if act_gelu else oracle.gelu_mul)(g, u)
+        assert oracle.rel_l2(ta.cpu().numpy(), other) > 1e-2, "the other activation fits as well: the test cannot tell them apart"
     want = oracle.gemm_truth(a, Wd, None, x)
     assert oracle.rel_l2(xt.cpu().numpy(), want) <= 3e-3
     ext_c.free_q_mlp(h)
     for l in (lg, lu, ld): l.unload()
+
+
+@pytest.mark.parametrize("rows", [1, 2, 8, 9, 13, 40])
+def test_q_mlp_block(rows):
+    _q_mlp_block(rows, False, False)
+
+
+@pytest.mark.parametrize("rows", [1, 2, 8, 9, 13, 40])
+@pytest.mark.parametrize("share_perm", [False, True], ids=["own_perm", "shared_perm"])
+def test_q_mlp_block_gelu(rows, share_perm):
+    _q_mlp_block(rows, True, False, share_perm)
+
+
+@pytest.mark.parametrize("act_gelu", [False, True])
+@pytest.mark.parametrize("rows", [1, 5, 12, 40])
+def test_q_mlp_block_bias(rows, act_gelu):
+    """gate / up linears with a bias: added in fp32 before the fp16 rounding that feeds the activation"""
+    _q_mlp_block(rows, act_gelu, True, share_perm=True)
