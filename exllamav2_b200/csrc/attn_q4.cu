@@ -1,4 +1,4 @@
-// Decode attention straight over the Q4 K/V cache: quantise-and-append the new rows, attend, in ONE kernel.
+// Decode attention straight over the Q4 / Q6 / Q8 K/V cache: quantise-and-append the new rows, attend, in ONE kernel.
 //
 // The reference runs, per layer and per step (exllamav2/attn.py:560-613, cache.py:472-556):
 //     q_to_fp16_kv over the WHOLE live cache -> flash_attn_with_kvcache on the fp16 temp -> fp16_to_q_kv of the new rows
@@ -9,6 +9,8 @@
 //         q . x = (H q) . y / 32            sum_s p_s x_s = H (sum_s p_s y_s) / 32
 //     the query is rotated ONCE, scores and the P V sum are formed on the stored (rotated) values, and the output is
 //     rotated back ONCE -- no per-position butterflies.
+//   * the kernel is templated on the element widths of keys (KB) and values (VB): (4, 4) is the Q4 cache, (8, 4) Q6 and
+//     (8, 8) Q8 (kvcache.cu).  An 8-bit row holds value e of a 32-value block at byte e, one fp16 scale per block as in Q4.
 //   * the q_len new K/V rows are quantised with exactly the arithmetic of fp16_to_q_kv (kvcache.cu pack_unit_q4, same
 //     bits as the reference) and written to the paged cache by one designated CTA per kv head.  The step that appends
 //     them attends them UNQUANTISED (fp16 values, rotated in fp32), exactly like the reference, where
@@ -32,7 +34,7 @@ struct AttnQ4Params {
     const half* q;          // [batch, q_len, H, hd]     (RoPE already applied)
     const half* k_new;      // [batch, q_len, KVH, hd]
     const half* v_new;
-    uint8_t* k_q;           // [pages, page_size, KVH, hd/2]
+    uint8_t* k_q;           // [pages, page_size, KVH, hd * KB / 8]
     half* k_s;              // [pages, page_size, KVH, hd/32]
     uint8_t* v_q;
     half* v_s;
@@ -54,8 +56,8 @@ struct AttnQ4Params {
     // and leaves (max, sum, unnormalised rotated output) in `ws`; the last to arrive (counter) merges.  Chunks are at least
     // AQ_SPLIT_MIN positions, so short contexts use one CTA and never touch the workspace.
     int sc_len;             // floats of the score buffer
-    int stage;              // cached positions per CTA copied to shared memory before the dependency wait (AQ_STAGE; AQ_STAGE / 2 with the ring)
-    int ring_slots;         // long contexts: cached rows beyond the staged window stream through a ring of AQ_SUB-position sub-chunks (0: loads from global)
+    int stage;              // cached positions per CTA copied to shared memory before the dependency wait (the bytes of AQ_STAGE Q4 rows; half with the ring)
+    int ring_slots;         // long contexts: cached rows beyond the staged window stream through a ring of sub-chunks (aq_sub) (0: loads from global)
     int batch;              // grid: one CTA per (head, sequence, split), flattened on x, padded to one CTA per SM with slot holders
     int busy_ctas;          //   = H * batch * nsplit
     unsigned int* slot_cnt; // CTAs of this launch that are done (self-resetting), see gemv_i8.cu
@@ -77,7 +79,8 @@ constexpr int AQ_SPLIT_MIN = 512;
 #define AQ_EXIT do { if (threadIdx.x == 0 && atomicAdd(P.slot_cnt, 1u) == gridDim.x - 1u) *reinterpret_cast<volatile unsigned int*>(P.slot_cnt) = 0u; return; } while (0)
 constexpr int AQ_SUB = 128;            // positions per sub-chunk of the streaming ring (long contexts)
 constexpr int AQ_RING = 4;             // sub-chunks in flight
-constexpr int AQ_STAGE = 512;          // cached positions per CTA staged in shared memory before the dependency wait
+constexpr int AQ_STAGE = 512;          // cached positions per CTA staged in shared memory before the dependency wait (Q4; the
+                                       // other formats stage the same number of BYTES, host side)
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
@@ -157,10 +160,19 @@ __device__ __forceinline__ int aq_dp4a_uu(uint32_t a, uint32_t b, int c) {
 
 // (nibble - 8) as fp32 without I2F: 0x4B000000 | n is the float 2^23 + n
 __device__ __forceinline__ float nib_f(uint32_t n) { return __uint_as_float(0x4B000000u | n) - 8388616.0f; }
+// (byte - 128) as fp32, same trick
+__device__ __forceinline__ float byte_f(uint32_t n) { return __uint_as_float(0x4B000000u | n) - 8388736.0f; }
 
-template <int HD>
+template <int KB, int VB>
+constexpr int aq_sub() { return AQ_SUB * 4 / (KB > VB ? KB : VB); }      // ring sub-chunk positions: the Q4 sub-chunk's bytes
+
+template <int HD, int KB, int VB>
 __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_constant__ AttnQ4Params P) {
-    constexpr int ROWB = HD / 2;            // packed bytes per (position, kv head)
+    static_assert((KB == 4 || KB == 8) && (VB == 4 || VB == 8), "element widths are 4 or 8 bits");
+    constexpr int ROWBK = HD * KB / 8;      // packed bytes per (position, kv head): keys
+    constexpr int ROWBV = HD * VB / 8;      //   values
+    constexpr int ROWB = ROWBK > ROWBV ? ROWBK : ROWBV;     // one ring slot position (keys, then values)
+    constexpr int SUB = aq_sub<KB, VB>();
     constexpr int NSC = HD / 32;            // scales per (position, kv head)
     constexpr int VEC = HD / 32;            // values per lane in the dims-on-lanes phase
     constexpr int UNITS = HD / 64;
@@ -178,17 +190,17 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
     float* qscl = reinterpret_cast<float*>(qsum + NSC);                    // [NSC]  its power-of-two scale
     float* red = qscl + NSC;                                               // [AQ_WARPS][HD]
     float* wred = red + AQ_WARPS * HD;                                     // [2 * AQ_WARPS]
-    uint8_t* new_q = reinterpret_cast<uint8_t*>(wred + 2 * AQ_WARPS);      // [2][AQ_MAX_QLEN][ROWB]
-    half* new_s = reinterpret_cast<half*>(new_q + 2 * AQ_MAX_QLEN * ROWB); // [2][AQ_MAX_QLEN][NSC]
+    uint8_t* new_q = reinterpret_cast<uint8_t*>(wred + 2 * AQ_WARPS);      // [AQ_MAX_QLEN][ROWBK], then [AQ_MAX_QLEN][ROWBV]
+    half* new_s = reinterpret_cast<half*>(new_q + AQ_MAX_QLEN * (ROWBK + ROWBV)); // [2][AQ_MAX_QLEN][NSC]
     float* new_y = reinterpret_cast<float*>(new_s + 2 * AQ_MAX_QLEN * NSC);// [2][AQ_MAX_QLEN][HD] rotated, unquantised new rows
     int* pages_s = reinterpret_cast<int*>(new_y + 2 * AQ_MAX_QLEN * HD);   // [pages_per_seq]
     float* sc = reinterpret_cast<float*>(pages_s + ((P.pages_per_seq + 3) & ~3));   // [sc_len]
-    uint8_t* kst = reinterpret_cast<uint8_t*>(sc + ((P.sc_len + 3) & ~3));            // [AQ_STAGE][ROWB]  staged cached K rows
-    uint8_t* vst = kst + P.stage * ROWB;                                             // [stage][ROWB]
-    half* ksst = reinterpret_cast<half*>(vst + P.stage * ROWB);                      // [stage][NSC]
+    uint8_t* kst = reinterpret_cast<uint8_t*>(sc + ((P.sc_len + 3) & ~3));            // [stage][ROWBK]  staged cached K rows
+    uint8_t* vst = kst + P.stage * ROWBK;                                            // [stage][ROWBV]
+    half* ksst = reinterpret_cast<half*>(vst + P.stage * ROWBV);                     // [stage][NSC]
     half* vsst = ksst + P.stage * NSC;
-    uint8_t* rq = reinterpret_cast<uint8_t*>(vsst + P.stage * NSC);                  // [AQ_RING][AQ_SUB][ROWB]  streaming ring (K, then V)
-    half* rs = reinterpret_cast<half*>(rq + AQ_RING * AQ_SUB * ROWB);                // [AQ_RING][AQ_SUB][NSC]
+    uint8_t* rq = reinterpret_cast<uint8_t*>(vsst + P.stage * NSC);                  // [AQ_RING][SUB][ROWB]  streaming ring (K, then V)
+    half* rs = reinterpret_cast<half*>(rq + AQ_RING * SUB * ROWB);                   // [AQ_RING][SUB][NSC]
 
     AQ_STAMP(0);
     griddep_launch_dependents();
@@ -220,19 +232,33 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
         p_hi = min(n_all, p_lo + chunk);
     }
     const int c_hi = min(p_hi, seqlen);          // cached rows of this CTA: [p_lo, c_hi)
-    // The first AQ_STAGE cached positions of this CTA are copied to shared memory with cp.async (no registers held across the
-    // wait): K / V nibbles [pos][ROWB] and their fp16 scales [pos][NSC].
+    // The first P.stage cached positions of this CTA are copied to shared memory with cp.async (no registers held across the
+    // wait): K / V elements [pos][ROWBK] / [pos][ROWBV] and their fp16 scales [pos][NSC].
     constexpr int TPR = NSC, RPP = AQ_THREADS / TPR;      // scores: NSC threads per position (one 32-value block + scale each)
     const int kblk = tid & (TPR - 1), krow = tid / TPR;
     const int n_st = max(0, min(c_hi - p_lo, P.stage));
     {
-        constexpr int CH = ROWB / 16;
-        for (int idx = tid; idx < n_st * CH; idx += AQ_THREADS) {
-            const int pos = idx / CH, ch = idx - pos * CH, pp = p_lo + pos;
-            const int page = btg[pp / P.page_size];
-            const size_t row = ((size_t)page * P.page_size + pp % P.page_size) * P.KVH + kvh;
-            cp_async16(smem_addr(kst + pos * ROWB + ch * 16), P.k_q + row * ROWB + ch * 16);
-            cp_async16(smem_addr(vst + pos * ROWB + ch * 16), P.v_q + row * ROWB + ch * 16);
+        if constexpr (ROWBK == ROWBV) {
+            constexpr int CH = ROWB / 16;
+            for (int idx = tid; idx < n_st * CH; idx += AQ_THREADS) {
+                const int pos = idx / CH, ch = idx - pos * CH, pp = p_lo + pos;
+                const int page = btg[pp / P.page_size];
+                const size_t row = ((size_t)page * P.page_size + pp % P.page_size) * P.KVH + kvh;
+                cp_async16(smem_addr(kst + pos * ROWB + ch * 16), P.k_q + row * ROWB + ch * 16);
+                cp_async16(smem_addr(vst + pos * ROWB + ch * 16), P.v_q + row * ROWB + ch * 16);
+            }
+        } else {
+            auto stage_rows = [&](uint8_t* dst, const uint8_t* src, auto rowb) {
+                constexpr int RB = decltype(rowb)::value, CH = RB / 16;
+                for (int idx = tid; idx < n_st * CH; idx += AQ_THREADS) {
+                    const int pos = idx / CH, ch = idx - pos * CH, pp = p_lo + pos;
+                    const int page = btg[pp / P.page_size];
+                    const size_t row = ((size_t)page * P.page_size + pp % P.page_size) * P.KVH + kvh;
+                    cp_async16(smem_addr(dst + pos * RB + ch * 16), src + row * RB + ch * 16);
+                }
+            };
+            stage_rows(kst, P.k_q, std::integral_constant<int, ROWBK>{});
+            stage_rows(vst, P.v_q, std::integral_constant<int, ROWBV>{});
         }
         for (int pos = tid; pos < n_st; pos += AQ_THREADS) {
             const int pp = p_lo + pos;
@@ -245,27 +271,29 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
     }
     for (int i = tid; i < P.pages_per_seq; i += AQ_THREADS) pages_s[i] = btg[i];
     const int* bt = pages_s;
-    // sub-chunk t of the cached rows beyond the staged window -> ring slot t % AQ_RING (one cp.async group per call, possibly empty)
-    auto ring_issue = [&](int t, const uint8_t* gq, const half* gs) {
-        const int base = p_lo + n_st + t * AQ_SUB, cnt = min(AQ_SUB, c_hi - base), slot = t & (AQ_RING - 1);
+    // sub-chunk t of the cached rows beyond the staged window -> ring slot t % AQ_RING (one cp.async group per call, possibly empty);
+    // rows of RB bytes (keys, then values) at a pitch of ROWB
+    auto ring_issue = [&](int t, const uint8_t* gq, const half* gs, auto rowb) {
+        constexpr int RB = decltype(rowb)::value;
+        const int base = p_lo + n_st + t * SUB, cnt = min(SUB, c_hi - base), slot = t & (AQ_RING - 1);
         if (cnt > 0) {
-            constexpr int CH = ROWB / 16;
+            constexpr int CH = RB / 16;
             for (int idx = tid; idx < cnt * CH; idx += AQ_THREADS) {
                 const int pos = idx / CH, ch = idx - pos * CH, pp = base + pos;
                 const int page = bt[pp / P.page_size];
                 const size_t row = ((size_t)page * P.page_size + pp % P.page_size) * P.KVH + kvh;
-                cp_async16(smem_addr(rq + (slot * AQ_SUB + pos) * ROWB + ch * 16), gq + row * ROWB + ch * 16);
+                cp_async16(smem_addr(rq + (slot * SUB + pos) * ROWB + ch * 16), gq + row * RB + ch * 16);
             }
             for (int pos = tid; pos < cnt; pos += AQ_THREADS) {
                 const int pp = base + pos;
                 const int page = bt[pp / P.page_size];
                 const size_t row = ((size_t)page * P.page_size + pp % P.page_size) * P.KVH + kvh;
-                cp_async_small<NSC * 2>(smem_addr(rs + (slot * AQ_SUB + pos) * NSC), gs + row * NSC);
+                cp_async_small<NSC * 2>(smem_addr(rs + (slot * SUB + pos) * NSC), gs + row * NSC);
             }
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
     };
-    const int ntail = (P.ring_slots && c_hi > p_lo + n_st) ? (c_hi - (p_lo + n_st) + AQ_SUB - 1) / AQ_SUB : 0;
+    const int ntail = (P.ring_slots && c_hi > p_lo + n_st) ? (c_hi - (p_lo + n_st) + SUB - 1) / SUB : 0;
     AQ_STAMP(1);
     griddep_wait();
     AQ_STAMP(2);
@@ -294,12 +322,24 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
         int sum = (int)(q0 + q1 - 2u * 0x4B400000u);
 #pragma unroll
         for (int o = 1; o < 16; o <<= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-        const int blk = e >> 5, l16 = lane & 15, j = l16 >> 2, m = l16 & 3;
-        uint8_t* qb = qi + blk * QIB + j * 16 + m;          // word order per j: even-high, even-low, odd-high, odd-low
-        qb[0] = (uint8_t)(q0 >> 8);
-        qb[4] = (uint8_t)q0;
-        qb[8] = (uint8_t)(q1 >> 8);
-        qb[12] = (uint8_t)q1;
+        const int blk = e >> 5, l16 = lane & 15;
+        if constexpr (KB == 4) {
+            const int j = l16 >> 2, m = l16 & 3;
+            uint8_t* qb = qi + blk * QIB + j * 16 + m;          // word order per j: even-high, even-low, odd-high, odd-low
+            qb[0] = (uint8_t)(q0 >> 8);
+            qb[4] = (uint8_t)q0;
+            qb[8] = (uint8_t)(q1 >> 8);
+            qb[12] = (uint8_t)q1;
+        } else {
+            // 8-bit keys: word w of a block holds values 4w..4w+3 in byte order; per pair of words j = w / 2 the 16 bytes are
+            // high(w = 2j), low(2j), high(2j + 1), low(2j + 1).  This lane's values 2 l16, 2 l16 + 1 sit in word l16 / 2.
+            const int w8 = l16 >> 1;
+            uint8_t* qb = qi + blk * QIB + (w8 >> 1) * 16 + (w8 & 1) * 8 + (l16 & 1) * 2;
+            qb[0] = (uint8_t)(q0 >> 8);
+            qb[1] = (uint8_t)(q1 >> 8);
+            qb[4] = (uint8_t)q0;
+            qb[5] = (uint8_t)q1;
+        }
         if (l16 == 0) {
             qsum[blk] = sum;
             qscl[blk] = amax > 0.f ? __uint_as_float((ef - 14u) << 23) : 0.f;
@@ -324,35 +364,66 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
         absmax = __hmax(absmax, __shfl_xor_sync(0xffffffffu, absmax, 4));
         absmax = __hmax(absmax, __shfl_xor_sync(0xffffffffu, absmax, 2));
         absmax = __hmax(absmax, __shfl_xor_sync(0xffffffffu, absmax, 1));
-        const half2 c_8 = __half2half2(__float2half_rn(8));
-        w2 = __h2div(w2, __half2half2(absmax));
-        w2 = __hfma2(w2, c_8, c_8);
-        const int q0 = min(max(__half2int_rn(__low2half(w2)), 0), 15);
-        const int q1 = min(max(__half2int_rn(__high2half(w2)), 0), 15);
-        new_q[(kv * AQ_MAX_QLEN + i) * ROWB + un * 32 + lane] = (uint8_t)(q0 | (q1 << 4));
-        if ((lane & 15) == 0) new_s[(kv * AQ_MAX_QLEN + i) * NSC + un * 2 + (lane >> 4)] = __hmul(absmax, __float2half_rn(1.0f / 8.0f));
+        uint8_t* nq = new_q + (kv ? AQ_MAX_QLEN * ROWBK + i * ROWBV : i * ROWBK);
+        if ((kv ? VB : KB) == 4) {
+            const half2 c_8 = __half2half2(__float2half_rn(8));
+            w2 = __h2div(w2, __half2half2(absmax));
+            w2 = __hfma2(w2, c_8, c_8);
+            const int q0 = min(max(__half2int_rn(__low2half(w2)), 0), 15);
+            const int q1 = min(max(__half2int_rn(__high2half(w2)), 0), 15);
+            nq[un * 32 + lane] = (uint8_t)(q0 | (q1 << 4));
+            if ((lane & 15) == 0) new_s[(kv * AQ_MAX_QLEN + i) * NSC + un * 2 + (lane >> 4)] = __hmul(absmax, __float2half_rn(1.0f / 8.0f));
+        } else {                                  // 8 bits (kvcache.cu pack_unit_q8)
+            const half2 c_128 = __half2half2(__float2half_rn(128));
+            w2 = __h2div(w2, __half2half2(absmax));
+            w2 = __hfma2(w2, c_128, c_128);
+            const int q0 = min(max(__half2int_rn(__low2half(w2)), 0), 255);
+            const int q1 = min(max(__half2int_rn(__high2half(w2)), 0), 255);
+            reinterpret_cast<uint16_t*>(nq + un * 64)[lane] = (uint16_t)(q0 | (q1 << 8));
+            if ((lane & 15) == 0) new_s[(kv * AQ_MAX_QLEN + i) * NSC + un * 2 + (lane >> 4)] = __hmul(absmax, __float2half_rn(1.0f / 128.0f));
+        }
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");
     __syncthreads();
     AQ_STAMP(3);
     AQ_STAMP(8);
 
-    // score of one 32-value block of a cached row (4-bit values, one fp16 scale) against its block of the rotated query:
-    // sum_d (nib_d - 8) q_d = sum nib q - 8 sum q, all in integers (dp4a on the masked words), one fp32 multiply at the end
-    auto score_blk = [&](uint4 kq, uint32_t ks) {
+    // score of one 32-value block of a cached row (one fp16 scale) against its block of the rotated query, all in integers (dp4a),
+    // one fp32 multiply at the end.  4 bits: sum_d (nib_d - 8) q_d = sum nib q - 8 sum q, dp4a on the masked words.
+    // 8 bits: sum_d (b_d - 128) q_d = sum b q - 128 sum q, dp4a on the stored words as they are.  The offset is removed with the
+    // block's query sum (one multiply-add per block, shared with the 4-bit path) rather than by flipping every byte's top bit and
+    // using signed dp4a (one extra logic op per word, 8 per block).
+    constexpr int KW = KB / 4;               // uint4 words per 32-value key block
+    constexpr uint32_t KFILL = KB == 4 ? 0x88888888u : 0x80808080u;      // a zero block (never scored: keeps registers defined)
+    auto score_blk = [&](const uint4* kq, uint32_t ks) {
         const uint8_t* qb = qi + kblk * QIB;
-        const uint32_t ww[4] = {kq.x, kq.y, kq.z, kq.w};
-        int a0 = 0, a1 = 0, a2 = 0, a3 = 0;
+        int v;
+        if constexpr (KB == 4) {
+            const uint32_t ww[4] = {kq[0].x, kq[0].y, kq[0].z, kq[0].w};
+            int a0 = 0, a1 = 0, a2 = 0, a3 = 0;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const uint4 qo = *reinterpret_cast<const uint4*>(qb + j * 16);
-            const uint32_t lo = ww[j] & 0x0f0f0f0fu, hi = ww[j] & 0xf0f0f0f0u;
-            a0 = aq_dp4a_us(lo, qo.x, a0);          // unsigned nibbles x signed high bytes
-            a1 = aq_dp4a_uu(lo, qo.y, a1);          // unsigned x unsigned low bytes
-            a2 = aq_dp4a_us(hi, qo.z, a2);
-            a3 = aq_dp4a_uu(hi, qo.w, a3);
+            for (int j = 0; j < 4; ++j) {
+                const uint4 qo = *reinterpret_cast<const uint4*>(qb + j * 16);
+                const uint32_t lo = ww[j] & 0x0f0f0f0fu, hi = ww[j] & 0xf0f0f0f0u;
+                a0 = aq_dp4a_us(lo, qo.x, a0);          // unsigned nibbles x signed high bytes
+                a1 = aq_dp4a_uu(lo, qo.y, a1);          // unsigned x unsigned low bytes
+                a2 = aq_dp4a_us(hi, qo.z, a2);
+                a3 = aq_dp4a_uu(hi, qo.w, a3);
+            }
+            v = ((a0 << 8) + a1) + (((a2 << 8) + a3) >> 4) - 8 * qsum[kblk];
+        } else {
+            const uint32_t ww[8] = {kq[0].x, kq[0].y, kq[0].z, kq[0].w, kq[1].x, kq[1].y, kq[1].z, kq[1].w};
+            int a0 = 0, a1 = 0, a2 = 0, a3 = 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const uint4 qo = *reinterpret_cast<const uint4*>(qb + j * 16);
+                a0 = aq_dp4a_us(ww[2 * j], qo.x, a0);          // unsigned bytes x signed high bytes
+                a1 = aq_dp4a_uu(ww[2 * j], qo.y, a1);          // unsigned x unsigned low bytes
+                a2 = aq_dp4a_us(ww[2 * j + 1], qo.z, a2);
+                a3 = aq_dp4a_uu(ww[2 * j + 1], qo.w, a3);
+            }
+            v = ((a0 + a2) << 8) + (a1 + a3) - 128 * qsum[kblk];
         }
-        const int v = ((a0 << 8) + a1) + (((a2 << 8) + a3) >> 4) - 8 * qsum[kblk];
         return __half2float(__ushort_as_half((unsigned short)ks)) * qscl[kblk] * (float)v;
     };
 
@@ -365,7 +436,7 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
 
         // ---- 2. scores: NSC threads per position, each its 32-value block of the (rotated) row against qrot ----
         float lmax = -INFINITY;
-        auto score_pos = [&](int p, uint4 kq, uint32_t ks) {      // warp-uniform call (the NSC partial sums meet by shuffle)
+        auto score_pos = [&](int p, const uint4* kq, uint32_t ks) {      // warp-uniform call (the NSC partial sums meet by shuffle)
             float s = 0.f;
             if (p < n_ctx) {
                 if (p >= seqlen) {               // a row appended by this step: fp16 values, rotated in fp32
@@ -397,15 +468,19 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
             int pb = p_lo;
             for (; pb < n_ctx && pb < st_end; pb += RPP) {
                 const int pp = pb + krow;
-                uint4 kq = make_uint4(0x88888888u, 0x88888888u, 0x88888888u, 0x88888888u);
+                uint4 kq[KW];
+#pragma unroll
+                for (int u = 0; u < KW; ++u) kq[u] = make_uint4(KFILL, KFILL, KFILL, KFILL);
                 uint32_t ks = 0u;
                 if (pp < st_end) {
-                    kq = *reinterpret_cast<const uint4*>(kst + (pp - p_lo) * ROWB + kblk * 16);
+#pragma unroll
+                    for (int u = 0; u < KW; ++u) kq[u] = reinterpret_cast<const uint4*>(kst + (pp - p_lo) * ROWBK)[kblk * KW + u];
                     ks = *reinterpret_cast<const unsigned short*>(ksst + (pp - p_lo) * NSC + kblk);
                 } else if (pp < min(n_ctx, seqlen)) {
                     const int page = bt[pp / P.page_size];
                     const size_t row = ((size_t)page * P.page_size + pp % P.page_size) * P.KVH + kvh;
-                    kq = __ldg(reinterpret_cast<const uint4*>(P.k_q + row * ROWB) + kblk);
+#pragma unroll
+                    for (int u = 0; u < KW; ++u) kq[u] = __ldg(reinterpret_cast<const uint4*>(P.k_q + row * ROWBK) + kblk * KW + u);
                     ks = __ldg(reinterpret_cast<const unsigned short*>(P.k_s + row * NSC) + kblk);
                 }
                 score_pos(pp, kq, ks);
@@ -413,45 +488,54 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
             if (ntail > 0) {
                 // long context: the remaining cached K rows stream through the ring, AQ_RING sub-chunks in flight
                 __syncthreads();                                  // (every thread is done with the ring's previous contents)
-                for (int t = 0; t < AQ_RING; ++t) ring_issue(t, P.k_q, P.k_s);
+                for (int t = 0; t < AQ_RING; ++t) ring_issue(t, P.k_q, P.k_s, std::integral_constant<int, ROWBK>{});
                 for (int t = 0; t < ntail; ++t) {
                     asm volatile("cp.async.wait_group %0;" ::"n"(AQ_RING - 1) : "memory");
                     __syncthreads();
-                    const int base = p_lo + n_st + t * AQ_SUB, slot = t & (AQ_RING - 1);
+                    const int base = p_lo + n_st + t * SUB, slot = t & (AQ_RING - 1);
 #pragma unroll 1
-                    for (int r0 = 0; r0 < AQ_SUB; r0 += RPP) {
+                    for (int r0 = 0; r0 < SUB; r0 += RPP) {
                         if (base + r0 >= n_ctx) break;
                         const int rr = r0 + krow, pp = base + rr;
-                        uint4 kq = make_uint4(0x88888888u, 0x88888888u, 0x88888888u, 0x88888888u);
+                        // an 8-bit sub-chunk can hold fewer positions than one pass scores (hd 64: 64 < RPP = 128): rows past
+                        // the sub-chunk belong to the next one and are neither read nor scored here
+                        const bool in_sub = SUB >= RPP || rr < SUB;
+                        uint4 kq[KW];
+#pragma unroll
+                        for (int u = 0; u < KW; ++u) kq[u] = make_uint4(KFILL, KFILL, KFILL, KFILL);
                         uint32_t ks = 0u;
-                        if (pp < c_hi) {
-                            kq = *reinterpret_cast<const uint4*>(rq + (slot * AQ_SUB + rr) * ROWB + kblk * 16);
-                            ks = *reinterpret_cast<const unsigned short*>(rs + (slot * AQ_SUB + rr) * NSC + kblk);
+                        if (in_sub && pp < c_hi) {
+#pragma unroll
+                            for (int u = 0; u < KW; ++u) kq[u] = reinterpret_cast<const uint4*>(rq + (slot * SUB + rr) * ROWB)[kblk * KW + u];
+                            ks = *reinterpret_cast<const unsigned short*>(rs + (slot * SUB + rr) * NSC + kblk);
                         }
-                        score_pos(pp, kq, ks);
+                        score_pos(in_sub ? pp : INT_MAX, kq, ks);
                     }
                     __syncthreads();
-                    ring_issue(t + AQ_RING, P.k_q, P.k_s);
+                    ring_issue(t + AQ_RING, P.k_q, P.k_s, std::integral_constant<int, ROWBK>{});
                 }
-                pb = p_lo + n_st + ntail * AQ_SUB;
+                pb = p_lo + n_st + ntail * SUB;
             }
-            for (; pb < n_ctx; pb += 2 * RPP) {                  // rows appended by this step; without the ring: everything beyond the window
-                uint4 kq[2];
-                uint32_t ks[2];
+            constexpr int TU = 2 / KW;                           // rows per thread in flight: 32 bytes of keys in every format
+            for (; pb < n_ctx; pb += TU * RPP) {                 // rows appended by this step; without the ring: everything beyond the window
+                uint4 kq[TU][KW];
+                uint32_t ks[TU];
 #pragma unroll
-                for (int u = 0; u < 2; ++u) {
+                for (int u = 0; u < TU; ++u) {
                     const int pp = pb + u * RPP + krow;
-                    kq[u] = make_uint4(0x88888888u, 0x88888888u, 0x88888888u, 0x88888888u);
+#pragma unroll
+                    for (int w = 0; w < KW; ++w) kq[u][w] = make_uint4(KFILL, KFILL, KFILL, KFILL);
                     ks[u] = 0u;
                     if (pp < min(n_ctx, seqlen)) {
                         const int page = bt[pp / P.page_size];
                         const size_t row = ((size_t)page * P.page_size + pp % P.page_size) * P.KVH + kvh;
-                        kq[u] = __ldg(reinterpret_cast<const uint4*>(P.k_q + row * ROWB) + kblk);
+#pragma unroll
+                        for (int w = 0; w < KW; ++w) kq[u][w] = __ldg(reinterpret_cast<const uint4*>(P.k_q + row * ROWBK) + kblk * KW + w);
                         ks[u] = __ldg(reinterpret_cast<const unsigned short*>(P.k_s + row * NSC) + kblk);
                     }
                 }
 #pragma unroll
-                for (int u = 0; u < 2; ++u)
+                for (int u = 0; u < TU; ++u)
                     if (pb + u * RPP < n_ctx) score_pos(pb + u * RPP + krow, kq[u], ks[u]);
             }
         }
@@ -482,7 +566,7 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
         float acc[VEC];
 #pragma unroll
         for (int j = 0; j < VEC; ++j) acc[j] = 0.f;
-        auto pv_fma = [&](uint32_t xs, float pw) {
+        auto pv_fma = [&](uint32_t xs, float pw) {                           // 4-bit values: nibbles | scale << 16
             const float pe = pw * __half2float(__ushort_as_half((unsigned short)(xs >> 16)));
             if constexpr (VEC == 4) {
                 acc[0] = fmaf(pe, nib_f(xs & 15u), acc[0]);
@@ -494,60 +578,89 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
                 acc[1] = fmaf(pe, nib_f((xs >> 4) & 15u), acc[1]);
             }
         };
+        auto pv_fma8 = [&](uint32_t xd, uint32_t xs, float pw) {             // 8-bit values: VEC bytes in xd, scale in xs
+            const float pe = pw * __half2float(__ushort_as_half((unsigned short)xs));
+#pragma unroll
+            for (int j = 0; j < VEC; ++j) acc[j] = fmaf(pe, byte_f((xd >> (8 * j)) & 0xffu), acc[j]);
+        };
+        auto v8_smem = [&](const uint8_t* rowp) -> uint32_t {               // this lane's VEC bytes of an 8-bit row
+            if constexpr (VEC == 4) return *reinterpret_cast<const uint32_t*>(rowp + lane * 4);
+            else return *reinterpret_cast<const uint16_t*>(rowp + lane * 2);
+        };
         {
             const int st_end = p_lo + n_st;                      // staged rows: shared memory
 #pragma unroll 4
             for (int p = p_lo + warp; p < st_end; p += AQ_WARPS) {
                 const int r = p - p_lo;
-                uint32_t x;
-                if constexpr (VEC == 4) x = *reinterpret_cast<const uint16_t*>(vst + r * ROWB + lane * 2);
-                else x = (uint32_t)vst[r * ROWB + lane] | 0x8800u;
-                x |= (uint32_t)(*reinterpret_cast<const uint16_t*>(vsst + r * NSC + ((lane * VEC) >> 5))) << 16;
-                pv_fma(x, sc[r]);
+                if constexpr (VB == 4) {
+                    uint32_t x;
+                    if constexpr (VEC == 4) x = *reinterpret_cast<const uint16_t*>(vst + r * ROWBV + lane * 2);
+                    else x = (uint32_t)vst[r * ROWBV + lane] | 0x8800u;
+                    x |= (uint32_t)(*reinterpret_cast<const uint16_t*>(vsst + r * NSC + ((lane * VEC) >> 5))) << 16;
+                    pv_fma(x, sc[r]);
+                } else {
+                    pv_fma8(v8_smem(vst + r * ROWBV), *reinterpret_cast<const uint16_t*>(vsst + r * NSC + ((lane * VEC) >> 5)), sc[r]);
+                }
             }
         }
         if (ntail > 0) {
             // long context: the remaining cached V rows through the same ring
             __syncthreads();
-            for (int t = 0; t < AQ_RING; ++t) ring_issue(t, P.v_q, P.v_s);
+            for (int t = 0; t < AQ_RING; ++t) ring_issue(t, P.v_q, P.v_s, std::integral_constant<int, ROWBV>{});
             for (int t = 0; t < ntail; ++t) {
                 asm volatile("cp.async.wait_group %0;" ::"n"(AQ_RING - 1) : "memory");
                 __syncthreads();
-                const int base = p_lo + n_st + t * AQ_SUB, slot = t & (AQ_RING - 1);
+                const int base = p_lo + n_st + t * SUB, slot = t & (AQ_RING - 1);
 #pragma unroll 4
-                for (int r = warp; r < AQ_SUB; r += AQ_WARPS) {
+                for (int r = warp; r < SUB; r += AQ_WARPS) {
                     const int pp = base + r;
                     if (pp < c_hi) {
-                        uint32_t x;
-                        if constexpr (VEC == 4) x = *reinterpret_cast<const uint16_t*>(rq + (slot * AQ_SUB + r) * ROWB + lane * 2);
-                        else x = (uint32_t)rq[(slot * AQ_SUB + r) * ROWB + lane] | 0x8800u;
-                        x |= (uint32_t)(*reinterpret_cast<const uint16_t*>(rs + (slot * AQ_SUB + r) * NSC + ((lane * VEC) >> 5))) << 16;
-                        pv_fma(x, sc[pp - p_lo]);
+                        const uint16_t xsc = *reinterpret_cast<const uint16_t*>(rs + (slot * SUB + r) * NSC + ((lane * VEC) >> 5));
+                        if constexpr (VB == 4) {
+                            uint32_t x;
+                            if constexpr (VEC == 4) x = *reinterpret_cast<const uint16_t*>(rq + (slot * SUB + r) * ROWB + lane * 2);
+                            else x = (uint32_t)rq[(slot * SUB + r) * ROWB + lane] | 0x8800u;
+                            x |= (uint32_t)xsc << 16;
+                            pv_fma(x, sc[pp - p_lo]);
+                        } else {
+                            pv_fma8(v8_smem(rq + (slot * SUB + r) * ROWB), xsc, sc[pp - p_lo]);
+                        }
                     }
                 }
                 __syncthreads();
-                ring_issue(t + AQ_RING, P.v_q, P.v_s);
+                ring_issue(t + AQ_RING, P.v_q, P.v_s, std::integral_constant<int, ROWBV>{});
             }
         }
         for (int p0 = (ntail > 0 ? c_hi : p_lo + n_st) + warp; p0 < c_hi; p0 += AQ_WARPS * 8) {   // without the ring: 8 rows in flight from global
-            uint32_t xs[8];
+            uint32_t xs[8], xd[VB == 8 ? 8 : 1];
 #pragma unroll
             for (int u = 0; u < 8; ++u) {
                 const int p = p0 + u * AQ_WARPS;
-                xs[u] = 0x8888u;
+                if constexpr (VB == 4) xs[u] = 0x8888u;
+                else { xs[u] = 0u; xd[u] = 0x80808080u; }
                 if (p < c_hi) {
                     const int page = bt[p / P.page_size];
                     const size_t row = ((size_t)page * P.page_size + p % P.page_size) * P.KVH + kvh;
-                    uint32_t x;
-                    if constexpr (VEC == 4) x = __ldg(reinterpret_cast<const uint16_t*>(P.v_q + row * ROWB + lane * 2));
-                    else x = (uint32_t)__ldg(P.v_q + row * ROWB + lane) | 0x8800u;
-                    xs[u] = x | ((uint32_t)__ldg(reinterpret_cast<const uint16_t*>(P.v_s + row * NSC + ((lane * VEC) >> 5))) << 16);
+                    if constexpr (VB == 4) {
+                        uint32_t x;
+                        if constexpr (VEC == 4) x = __ldg(reinterpret_cast<const uint16_t*>(P.v_q + row * ROWBV + lane * 2));
+                        else x = (uint32_t)__ldg(P.v_q + row * ROWBV + lane) | 0x8800u;
+                        xs[u] = x | ((uint32_t)__ldg(reinterpret_cast<const uint16_t*>(P.v_s + row * NSC + ((lane * VEC) >> 5))) << 16);
+                    } else {
+                        const uint32_t xsc = __ldg(reinterpret_cast<const uint16_t*>(P.v_s + row * NSC + ((lane * VEC) >> 5)));
+                        if constexpr (VEC == 4) xd[u] = __ldg(reinterpret_cast<const uint32_t*>(P.v_q + row * ROWBV) + lane);
+                        else xd[u] = __ldg(reinterpret_cast<const uint16_t*>(P.v_q + row * ROWBV) + lane);
+                        xs[u] = xsc;
+                    }
                 }
             }
 #pragma unroll
             for (int u = 0; u < 8; ++u) {
                 const int p = p0 + u * AQ_WARPS;
-                if (p < c_hi) pv_fma(xs[u], sc[p - p_lo]);
+                if (p < c_hi) {
+                    if constexpr (VB == 4) pv_fma(xs[u], sc[p - p_lo]);
+                    else pv_fma8(xd[u], xs[u], sc[p - p_lo]);
+                }
             }
         }
         if (warp == 0) {                                                      // rows appended by this step (<= 8)
@@ -565,14 +678,27 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
         // the rows appended by this step go to the cache now, from shared memory, by the last warp (it has no part in the reduction
         // below): nothing on the way to the output waits for these stores
         if (i == P.q_len - 1 && warp == AQ_WARPS - 1 && h % group == 0 && z == 0) {
-            for (int idx = lane; idx < 2 * P.q_len * (ROWB / 4); idx += 32) {
-                const int kv = idx / (P.q_len * (ROWB / 4)), r = idx - kv * P.q_len * (ROWB / 4);
-                const int ii = r / (ROWB / 4), wd = r - ii * (ROWB / 4);
-                const int pos = seqlen + ii;
-                const int page = bt[pos / P.page_size];
-                const size_t row = ((size_t)page * P.page_size + pos % P.page_size) * P.KVH + kvh;
-                reinterpret_cast<uint32_t*>((kv ? P.v_q : P.k_q) + row * ROWB)[wd] =
-                    reinterpret_cast<const uint32_t*>(new_q + (kv * AQ_MAX_QLEN + ii) * ROWB)[wd];
+            if constexpr (ROWBK == ROWBV) {
+                for (int idx = lane; idx < 2 * P.q_len * (ROWB / 4); idx += 32) {
+                    const int kv = idx / (P.q_len * (ROWB / 4)), r = idx - kv * P.q_len * (ROWB / 4);
+                    const int ii = r / (ROWB / 4), wd = r - ii * (ROWB / 4);
+                    const int pos = seqlen + ii;
+                    const int page = bt[pos / P.page_size];
+                    const size_t row = ((size_t)page * P.page_size + pos % P.page_size) * P.KVH + kvh;
+                    reinterpret_cast<uint32_t*>((kv ? P.v_q : P.k_q) + row * ROWB)[wd] =
+                        reinterpret_cast<const uint32_t*>(new_q + (kv * AQ_MAX_QLEN + ii) * ROWB)[wd];
+                }
+            } else {
+                constexpr int WK = ROWBK / 4, WV = ROWBV / 4;                 // 32-bit words per key / value row
+                for (int idx = lane; idx < P.q_len * (WK + WV); idx += 32) {
+                    const int kv = idx >= P.q_len * WK, r = kv ? idx - P.q_len * WK : idx;
+                    const int ii = kv ? r / WV : r / WK, wd = kv ? r - ii * WV : r - ii * WK;
+                    const int pos = seqlen + ii;
+                    const int page = bt[pos / P.page_size];
+                    const size_t row = ((size_t)page * P.page_size + pos % P.page_size) * P.KVH + kvh;
+                    reinterpret_cast<uint32_t*>(kv ? P.v_q + row * ROWBV : P.k_q + row * ROWBK)[wd] =
+                        reinterpret_cast<const uint32_t*>(new_q + (kv ? AQ_MAX_QLEN * ROWBK + ii * ROWBV : ii * ROWBK))[wd];
+                }
             }
             for (int idx = lane; idx < 2 * P.q_len * NSC; idx += 32) {
                 const int kv = idx / (P.q_len * NSC), r = idx - kv * P.q_len * NSC;
@@ -707,7 +833,36 @@ extern "C" int exl2b_paged_attn_decode_q4_ex(const uint16_t* q, const uint16_t* 
                                              int num_kv_heads, int head_dim, int page_size, int pages_per_seq, float softmax_scale,
                                              exl2b_qmatrix_t out_consumer, const uint16_t* rope_sin, const uint16_t* rope_cos,
                                              int rope_style, int sincos_size, exl2b_stream_t stream) {
+    return exl2b_paged_attn_decode_q(q, k_new, v_new, k_cache, k_scales, v_cache, v_scales, cache_seqlens, block_table, out, batch, q_len,
+                                     num_heads, num_kv_heads, head_dim, page_size, pages_per_seq, softmax_scale, out_consumer, rope_sin,
+                                     rope_cos, rope_style, sincos_size, 4, stream);
+}
+
+template <int KB, int VB>
+static int attn_q_launch(int head_dim, dim3 grid, size_t smem, cudaStream_t stream, const AttnQ4Params& P) {
+    if (head_dim == 128)
+        EXL2B_CUDA(launch_pdl_f("attn", attn_q4_kernel<128, KB, VB>, grid, dim3(AQ_THREADS), smem, stream, P));
+    else
+        EXL2B_CUDA(launch_pdl_f("attn", attn_q4_kernel<64, KB, VB>, grid, dim3(AQ_THREADS), smem, stream, P));
+    return 0;
+}
+
+template <int KB, int VB>
+static int attn_q_set_smem() {
+    EXL2B_CUDA(cudaFuncSetAttribute(attn_q4_kernel<128, KB, VB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    EXL2B_CUDA(cudaFuncSetAttribute(attn_q4_kernel<64, KB, VB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    return 0;
+}
+
+extern "C" int exl2b_paged_attn_decode_q(const uint16_t* q, const uint16_t* k_new, const uint16_t* v_new, uint8_t* k_cache,
+                                         uint16_t* k_scales, uint8_t* v_cache, uint16_t* v_scales, const int32_t* cache_seqlens,
+                                         const int32_t* block_table, uint16_t* out, int batch, int q_len, int num_heads,
+                                         int num_kv_heads, int head_dim, int page_size, int pages_per_seq, float softmax_scale,
+                                         exl2b_qmatrix_t out_consumer, const uint16_t* rope_sin, const uint16_t* rope_cos,
+                                         int rope_style, int sincos_size, int wbits, exl2b_stream_t stream) {
     EXL2B_REQUIRE(q && k_new && v_new && k_cache && k_scales && v_cache && v_scales && cache_seqlens && block_table && out, "null argument");
+    EXL2B_REQUIRE(wbits == 4 || wbits == 6 || wbits == 8, "cache wbits must be 4 (Q4), 6 (Q6) or 8 (Q8); got %d", wbits);
+    const int kb = wbits == 4 ? 4 : 8, vb = wbits == 8 ? 8 : 4;
     EXL2B_REQUIRE(head_dim == 64 || head_dim == 128, "head_dim %d not supported (64 or 128)", head_dim);
     EXL2B_REQUIRE(num_heads % num_kv_heads == 0, "bad GQA ratio");
     EXL2B_REQUIRE(q_len >= 1 && q_len <= AQ_MAX_QLEN, "q_len %d outside the decode regime (1..%d)", q_len, AQ_MAX_QLEN);
@@ -781,21 +936,29 @@ extern "C" int exl2b_paged_attn_decode_q4_ex(const uint16_t* q, const uint16_t* 
     const int sc_len = nsplit > 1 ? std::max(AQ_SPLIT_MIN, (P.max_ctx + nsplit) / nsplit) + 8 : P.max_ctx + q_len;
     const int hd = head_dim;
     P.sc_len = sc_len;
-    // cached rows beyond the staged window: streamed through a ring of 4 x 128 positions when the cache is long; the ring takes the
-    // place of half the staged window, so the CTA keeps the footprint that lets it share an SM with one GEMV CTA (a first version
-    // that ADDED the ring lost that co-residency).  The ring pays once a CTA has thousands of positions; below, the larger window
-    // wins.  The host only knows the cache's capacity:
+    // cached rows beyond the staged window: streamed through a ring of 4 sub-chunks (128 positions at Q4) when the cache is long;
+    // the ring takes the place of half the staged window, so the CTA keeps the footprint that lets it share an SM with one GEMV
+    // CTA (a first version that ADDED the ring lost that co-residency).  The ring pays once a CTA has thousands of positions;
+    // below, the larger window wins.  The host only knows the cache's capacity:
     P.ring_slots = (P.max_ctx > 8192) ? AQ_RING : 0;
-    P.stage = P.ring_slots ? AQ_STAGE / 2 : AQ_STAGE;          // (the ring takes the place of half the window: same footprint)
-    const size_t smem = (size_t)((hd / 32) * 36 + AQ_WARPS * hd + 2 * AQ_WARPS) * 4 + (size_t)(hd / 32) * (80 + 8) + 2 * AQ_MAX_QLEN * (hd / 2) + 2 * AQ_MAX_QLEN * (hd / 32) * 2 +
+    // The window and the ring are sized in BYTES: every format stages at most the bytes of Q4's AQ_STAGE (or AQ_STAGE / 2 with
+    // the ring) positions, in whole multiples of 64 positions, so no format needs more shared memory than Q4: Q8 stages 256
+    // (128) positions, Q6 320 (128).  Ring sub-chunks hold the bytes of 128 Q4 rows of the wider of K and V (64 at 8 bits).
+    const int rowk = hd * kb / 8, rowv = hd * vb / 8, nsc = hd / 32;
+    const int window = P.ring_slots ? AQ_STAGE / 2 : AQ_STAGE;
+    P.stage = (int)((size_t)window * (hd + 4 * nsc) / (size_t)(rowk + rowv + 4 * nsc)) / 64 * 64;
+    const int sub = AQ_SUB * 4 / std::max(kb, vb);
+    const size_t smem = (size_t)((hd / 32) * 36 + AQ_WARPS * hd + 2 * AQ_WARPS) * 4 + (size_t)(hd / 32) * (80 + 8) + AQ_MAX_QLEN * (rowk + rowv) + 2 * AQ_MAX_QLEN * (hd / 32) * 2 +
                         (size_t)2 * AQ_MAX_QLEN * hd * 4 + (size_t)((pages_per_seq + 3) & ~3) * 4 + (size_t)((sc_len + 3) & ~3) * 4 +
-                        (size_t)P.stage * (hd / 2) * 2 + (size_t)P.stage * (hd / 32) * 2 * 2 +
-                        (P.ring_slots ? (size_t)AQ_RING * AQ_SUB * (hd / 2 + (hd / 32) * 2) : 0);
+                        (size_t)P.stage * (rowk + rowv) + (size_t)P.stage * nsc * 2 * 2 +
+                        (P.ring_slots ? (size_t)AQ_RING * sub * (std::max(rowk, rowv) + nsc * 2) : 0);
     EXL2B_REQUIRE(smem <= 200 * 1024, "context of %d tokens does not fit the score buffer", P.max_ctx);
     static bool attr_set[64] = {false};
     if (!attr_set[dev]) {
-        EXL2B_CUDA(cudaFuncSetAttribute(attn_q4_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        EXL2B_CUDA(cudaFuncSetAttribute(attn_q4_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        int rc = attn_q_set_smem<4, 4>();
+        if (!rc) rc = attn_q_set_smem<8, 4>();
+        if (!rc) rc = attn_q_set_smem<8, 8>();
+        if (rc) return rc;
         attr_set[dev] = true;
     }
     static unsigned int* slot_cnts[64] = {nullptr};
@@ -808,9 +971,7 @@ extern "C" int exl2b_paged_attn_decode_q4_ex(const uint16_t* q, const uint16_t* 
     P.batch = batch;
     P.busy_ctas = num_heads * batch * nsplit;
     dim3 grid(slot_holders_disabled() ? P.busy_ctas : std::max(P.busy_ctas, device_sm_count(dev)));
-    if (head_dim == 128)
-        EXL2B_CUDA(launch_pdl_f("attn", attn_q4_kernel<128>, grid, dim3(AQ_THREADS), smem, (cudaStream_t)stream, P));
-    else
-        EXL2B_CUDA(launch_pdl_f("attn", attn_q4_kernel<64>, grid, dim3(AQ_THREADS), smem, (cudaStream_t)stream, P));
-    return 0;
+    if (wbits == 4) return attn_q_launch<4, 4>(head_dim, grid, smem, (cudaStream_t)stream, P);
+    if (wbits == 6) return attn_q_launch<8, 4>(head_dim, grid, smem, (cudaStream_t)stream, P);
+    return attn_q_launch<8, 8>(head_dim, grid, smem, (cudaStream_t)stream, P);
 }

@@ -90,6 +90,7 @@ _sig("exl2b_qmlp_forward", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
 _sig("exl2b_qmlp_forward_gateup", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p)
 _sig("exl2b_paged_attn_decode_q4", c_int, *([c_void_p] * 10 + [c_int] * 7 + [c_float, c_void_p, c_void_p]))
 _sig("exl2b_paged_attn_decode_q4_ex", c_int, *([c_void_p] * 10 + [c_int] * 7 + [c_float, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]))
+_sig("exl2b_paged_attn_decode_q", c_int, *([c_void_p] * 10 + [c_int] * 7 + [c_float, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]))
 _sig("exl2b_paged_attn_status", c_int, c_int, POINTER(c_int))
 _sig("exl2b_paged_attn_clear_status", c_int, c_int)
 
@@ -321,8 +322,24 @@ def act_mul(x: torch.Tensor, y: torch.Tensor, act_gelu: bool = False):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# Q4 K/V cache
+# Q4 / Q6 / Q8 K/V cache
 # ---------------------------------------------------------------------------------------------------------------
+
+# values per stored byte of the keys / values for each cache format (cache.py:584-656): Q4 2/2, Q6 1/2, Q8 1/1
+KV_WEIGHTS_PER_BYTE = {4: (2, 2), 6: (1, 2), 8: (1, 1)}
+
+
+def _check_kv_shapes(fp16_k, q_k, fp16_v, q_v, wbits):
+    """The kernel derives every offset from the fp16 tensor's shape: a quantised state tensor of the wrong width for `wbits`
+    would be read or written out of bounds.  (An unknown wbits is left to the library, whose error names the accepted ones.)"""
+    if wbits not in KV_WEIGHTS_PER_BYTE:
+        return
+    for name, f, q, wpe in (("key", fp16_k, q_k, KV_WEIGHTS_PER_BYTE[wbits][0]), ("value", fp16_v, q_v, KV_WEIGHTS_PER_BYTE[wbits][1])):
+        if f is None or f.is_meta or q is None or q.is_meta:
+            continue
+        if q.shape[-1] * wpe != f.shape[-1]:
+            raise RuntimeError(f"{name} states have last dimension {q.shape[-1]}, but a wbits={wbits} cache stores "
+                               f"{f.shape[-1] // wpe} bytes per {f.shape[-1]}-value row")
 
 def _kv_call(fn, a_k, b_k, s_k, a_v, b_v, s_v, fp16_k, batch_size, offset, width, page_size, cache_seqlens, block_table, wbits):
     dim = fp16_k.shape[2] * fp16_k.shape[3]
@@ -343,6 +360,7 @@ def fp16_to_q_kv(k_in, k_out, k_scales, v_in, v_out, v_scales, batch_size: int, 
     _cuda(k_in, "k_in")
     _dtype(k_in, torch.float16, "k_in")
     _dtype(k_out, torch.uint8, "k_out")
+    _check_kv_shapes(k_in, k_out, v_in, v_out, wbits)
     _kv_call(lib.exl2b_fp16_to_q_kv, k_in, k_out, k_scales, v_in, v_out, v_scales, k_in, batch_size, offset, width,
              page_size, cache_seqlens, block_table, wbits)
 
@@ -353,6 +371,7 @@ def q_to_fp16_kv(k_in, k_out, k_scales, v_in, v_out, v_scales, batch_size: int, 
     _cuda(k_in, "k_in")
     _dtype(k_in, torch.uint8, "k_in")
     _dtype(k_out, torch.float16, "k_out")
+    _check_kv_shapes(k_out, k_in, v_out, v_in, wbits)
     # C ABI order is (in, scales, out)
     dim = k_out.shape[2] * k_out.shape[3]
     seq_stride = k_out.shape[1] * dim
@@ -521,22 +540,23 @@ def gemm_half_q_half_prepared(b: int, c, has_norm: bool, norm_eps: float, clear:
 
 
 def paged_attn_decode_q4(q, k_new, v_new, k_cache, k_scales, v_cache, v_scales, cache_seqlens, block_table, out,
-                         softmax_scale: float, out_consumer: int = 0, rope=None):
-    """Decode attention over the paged Q4 cache with quantise-and-append of the new rows (include/exl2_b200.h
-    exl2b_paged_attn_decode_q4).  q [B, q_len, H, hd]; k_new / v_new [B, q_len, KVH, hd]; caches uint8
-    [pages, page, KVH, hd/2] + fp16 scales [pages, page, KVH, hd/32]; out like q.  No reference counterpart as one op:
-    it replaces q_to_fp16_kv + flash_attn_with_kvcache + fp16_to_q_kv (attn.py:560-613)."""
+                         softmax_scale: float, out_consumer: int = 0, rope=None, wbits: int = 4):
+    """Decode attention over the paged Q4 / Q6 / Q8 cache (`wbits` as fp16_to_q_kv) with quantise-and-append of the new rows
+    (include/exl2_b200.h exl2b_paged_attn_decode_q).  q [B, q_len, H, hd]; k_new / v_new [B, q_len, KVH, hd]; caches uint8
+    [pages, page, KVH, hd/2] (4-bit) or [pages, page, KVH, hd] (8-bit) + fp16 scales [pages, page, KVH, hd/32]; out like q.
+    No reference counterpart as one op: it replaces q_to_fp16_kv + flash_attn_with_kvcache + fp16_to_q_kv (attn.py:560-613)."""
     B, q_len, H, hd = q.shape
     KVH = k_new.shape[2]
     for t in (q, k_new, v_new, out):
         _dtype(_cuda(t, "attention operand"), torch.half, "attention operand")
+    _check_kv_shapes(k_new, k_cache, v_new, v_cache, wbits)
     # rope = (sin, cos, rope_style): q / k_new are the un-rotated projection outputs, rotated as the kernel reads them
     sin, cos, style = rope if rope is not None else (None, None, 0)
-    _check(lib.exl2b_paged_attn_decode_q4_ex(
+    _check(lib.exl2b_paged_attn_decode_q(
         _p(q), _p(k_new), _p(v_new), _p(k_cache), _p(k_scales), _p(v_cache), _p(v_scales),
         _p(cache_seqlens), _p(block_table), _p(out), B, q_len, H, KVH, hd, k_cache.shape[1], block_table.shape[1],
         float(softmax_scale), out_consumer or None, _p(sin), _p(cos), int(style), sin.shape[-1] if sin is not None else 0,
-        _stream(q)))
+        int(wbits), _stream(q)))
 
 
 def paged_attn_clear_status(device) -> None:

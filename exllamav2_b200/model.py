@@ -1,6 +1,6 @@
 """Llama-family decode graph over the drop-in operator surface -- the host-side mirror of the reference's module
 loop for quantized models (exllamav2/model.py:938-1054 forward_chunk; attn.py:466-638 forward_paged; mlp.py:318-358;
-cache.py:306-606 ExLlamaV2Cache_Q4), used by bench.py and the end-to-end tests.
+cache.py:306-656 ExLlamaV2Cache_Q4 / _Q6 / _Q8), used by bench.py and the end-to-end tests.
 
 Per decoder layer the call sequence is exactly the reference's:
     cache.get_kv_state (q_to_fp16_kv)  ->  ext_c.q_attn_forward_1  ->  paged attention with kv-append
@@ -89,9 +89,12 @@ def rope_tables(head_dim: int, max_seq_len: int, base: float, device) -> tuple[t
     return emb.sin().half(), emb.cos().half()
 
 
-class ExLlamaV2Cache_Q4:
-    """Q4 K/V cache (cache.py:306-606): uint8 nibbles + fp16 scales per 32 values, plus ONE shared fp16 temp pair that
-    get_kv_state fills for the layer being evaluated (cache.py:464-469)."""
+class ExLlamaV2Cache_Q:
+    """Quantised K/V cache (cache.py:306-606): uint8 elements + fp16 scales per 32 values, plus ONE shared fp16 temp pair that
+    get_kv_state fills for the layer being evaluated (cache.py:464-469).  `wbits` selects the format as in the reference:
+    4 = Q4 (4-bit keys and values), 6 = Q6 (8-bit keys, 4-bit values), 8 = Q8 (8-bit keys and values)."""
+
+    wbits = 4
 
     def __init__(self, cfg: LlamaConfig, batch_size: int, max_seq_len: int, device):
         assert max_seq_len % PAGE_SIZE == 0
@@ -100,8 +103,9 @@ class ExLlamaV2Cache_Q4:
         self.pages = batch_size * max_seq_len // PAGE_SIZE
         kvh, hd = cfg.num_kv_heads, cfg.head_dim
         shp = (self.pages, PAGE_SIZE, kvh, hd)
-        self.key_states = [torch.zeros(shp[:3] + (hd // 2,), dtype=torch.uint8, device=device) for _ in range(cfg.num_layers)]
-        self.value_states = [torch.zeros_like(self.key_states[0]) for _ in range(cfg.num_layers)]
+        wpe_k, wpe_v = ext_c.KV_WEIGHTS_PER_BYTE[self.wbits]          # values per byte, cache.py:66-69
+        self.key_states = [torch.zeros(shp[:3] + (hd // wpe_k,), dtype=torch.uint8, device=device) for _ in range(cfg.num_layers)]
+        self.value_states = [torch.zeros(shp[:3] + (hd // wpe_v,), dtype=torch.uint8, device=device) for _ in range(cfg.num_layers)]
         self.key_scales = [torch.zeros(shp[:3] + (hd // 32,), dtype=torch.half, device=device) for _ in range(cfg.num_layers)]
         self.value_scales = [torch.zeros_like(self.key_scales[0]) for _ in range(cfg.num_layers)]
         self.temp_k = torch.zeros(shp, dtype=torch.half, device=device)
@@ -114,17 +118,32 @@ class ExLlamaV2Cache_Q4:
         """cache.py:472-514: dequantise the live part of the layer's cache into the fp16 temp (paged form)."""
         ext_c.q_to_fp16_kv(self.key_states[layer], self.temp_k, self.key_scales[layer],
                            self.value_states[layer], self.temp_v, self.value_scales[layer],
-                           self.batch_size, 0, 0, PAGE_SIZE, self.cache_seqlens, self.block_table, 4)
+                           self.batch_size, 0, 0, PAGE_SIZE, self.cache_seqlens, self.block_table, self.wbits)
         return self.temp_k, self.temp_v
 
     def store_kv_state(self, layer: int, q_len: int):
         """cache.py:517-556: quantise the q_len tokens appended at [seqlen, seqlen + q_len)."""
         ext_c.fp16_to_q_kv(self.temp_k, self.key_states[layer], self.key_scales[layer],
                            self.temp_v, self.value_states[layer], self.value_scales[layer],
-                           self.batch_size, 0, q_len, PAGE_SIZE, self.cache_seqlens, self.block_table, 4)
+                           self.batch_size, 0, q_len, PAGE_SIZE, self.cache_seqlens, self.block_table, self.wbits)
 
     def footprint(self) -> int:
         return sum(t.numel() * t.element_size() for ts in (self.key_states, self.value_states, self.key_scales, self.value_scales) for t in ts)
+
+
+class ExLlamaV2Cache_Q4(ExLlamaV2Cache_Q):
+    wbits = 4
+
+
+class ExLlamaV2Cache_Q6(ExLlamaV2Cache_Q):
+    wbits = 6
+
+
+class ExLlamaV2Cache_Q8(ExLlamaV2Cache_Q):
+    wbits = 8
+
+
+CACHE_CLASSES = {4: ExLlamaV2Cache_Q4, 6: ExLlamaV2Cache_Q6, 8: ExLlamaV2Cache_Q8}
 
 
 _FA = [False, None]
@@ -181,7 +200,10 @@ class _Layer:
 class ExLlamaV2Decoder:
     """Quantized Llama decoder: embedding -> L x (attention block, MLP block) -> norm -> lm_head."""
 
-    def __init__(self, cfg: LlamaConfig, device="cuda:0", seed: int = 0, batch_size: int = 1, cache_len: int | None = None):
+    def __init__(self, cfg: LlamaConfig, device="cuda:0", seed: int = 0, batch_size: int = 1, cache_len: int | None = None,
+                 cache_bits: int = 4):
+        if cache_bits not in CACHE_CLASSES:
+            raise ValueError(f"cache_bits must be 4 (Q4), 6 (Q6) or 8 (Q8); got {cache_bits}")
         self.cfg, self.device = cfg, torch.device(device)
         dev = self.device
         H, KVH, hd, hid, inter = cfg.num_heads, cfg.num_kv_heads, cfg.head_dim, cfg.hidden_size, cfg.intermediate_size
@@ -227,7 +249,7 @@ class ExLlamaV2Decoder:
         # one table row per cache position: the fused / stand-alone RoPE kernels index the tables by position and cannot see their length
         cache_len = cache_len or min(cfg.max_seq_len, 1024)
         self.sin, self.cos = rope_tables(hd, max(cfg.max_seq_len, (cache_len + 255) // 256 * 256), cfg.rope_theta, dev)
-        self.cache = ExLlamaV2Cache_Q4(cfg, batch_size, cache_len, dev)
+        self.cache = CACHE_CLASSES[cache_bits](cfg, batch_size, cache_len, dev)
         self.batch_size = batch_size
         # static decode buffers (graph-capturable)
         B = batch_size
@@ -241,7 +263,7 @@ class ExLlamaV2Decoder:
         self.logits = torch.empty((B, cfg.vocab_size), dtype=torch.half, device=dev)
         self.graph = None
         self.pos = 0        # host-side mirror of cache_seqlens (which lives on the device): bounds are checked BEFORE a launch
-        # True: attention reads the Q4 cache directly (one kernel per layer); False: the reference's sequence
+        # True: attention reads the quantised cache directly (one kernel per layer); False: the reference's sequence
         # q_to_fp16_kv -> attention on the fp16 temp -> fp16_to_q_kv (three kernels + the temp round trip)
         self.fused_attn = os.environ.get("EXL2B_REF_KV_SEQUENCE") is None
         # producer epilogues feed consumer activation buffers (needs the default LAYOUT_TC matrix layout)
@@ -268,7 +290,7 @@ class ExLlamaV2Decoder:
                 ext_c.paged_attn_decode_q4(q.view(B, q_len, H, hd), k.view(B, q_len, KVH, hd), v.view(B, q_len, KVH, hd),
                                            cache.key_states[li], cache.key_scales[li], cache.value_states[li],
                                            cache.value_scales[li], cache.cache_seqlens, cache.block_table,
-                                           attn_out.view(B, q_len, H, hd), 1.0 / math.sqrt(hd))
+                                           attn_out.view(B, q_len, H, hd), 1.0 / math.sqrt(hd), wbits=cache.wbits)
                 ext_c.q_attn_forward_2(L.attn, x, attn_out, B, q_len)
                 ext_c.q_mlp_forward_(L.mlp, x)
                 continue
@@ -287,7 +309,7 @@ class ExLlamaV2Decoder:
 
     def _forward_tokens_chained(self, x, q, k, v, attn_out, q_len: int, head: bool = False, gemv_only: bool = False):
         """Same layer loop with every producer's epilogue feeding its consumer's activation buffer (include/exl2_b200.h
-        "chained launches"): 5 launches per layer -- QKV(+norm+rope), attention over the Q4 cache, O(+residual),
+        "chained launches"): 5 launches per layer -- QKV(+norm+rope), attention over the quantised cache, O(+residual),
         gate|up(+norm+act), down(+residual) -- and no stand-alone norm / rope / prep / cache kernels."""
         cfg, cache = self.cfg, self.cache
         B = self.batch_size
@@ -303,7 +325,7 @@ class ExLlamaV2Decoder:
                                            cache.key_states[li], cache.key_scales[li], cache.value_states[li],
                                            cache.value_scales[li], cache.cache_seqlens, cache.block_table,
                                            attn_out.view(B, q_len, H, hd), 1.0 / math.sqrt(hd), L.o_proj.q_handle,
-                                           rope=(self.sin, self.cos, 2) if fuse_rope else None)
+                                           rope=(self.sin, self.cos, 2) if fuse_rope else None, wbits=cache.wbits)
             ext_c.q_attn_forward_2_ex(L.attn, x, attn_out, B, q_len, True, L.chain_mlp)
             if li + 1 < n:
                 nxt = self.layers[li + 1].chain_attn
