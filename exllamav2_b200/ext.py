@@ -341,7 +341,18 @@ def _check_kv_shapes(fp16_k, q_k, fp16_v, q_v, wbits):
             raise RuntimeError(f"{name} states have last dimension {q.shape[-1]}, but a wbits={wbits} cache stores "
                                f"{f.shape[-1] // wpe} bytes per {f.shape[-1]}-value row")
 
+def _check_kv_range(fp16_k, batch_size: int, offset: int, width: int, page_size: int):
+    """Non-paged: tokens [offset, offset + width) of `batch_size` rows must lie inside the fp16 tensor; the kernels then widen
+    the range to whole 512-value blocks within each row and never past its end (kvcache.cu kv_common)."""
+    if page_size:
+        return
+    if batch_size > fp16_k.shape[0] or offset < 0 or width < 0 or offset + width > fp16_k.shape[1]:
+        raise RuntimeError(f"tokens [{offset}, {offset + width}) of {batch_size} rows are outside the tensor's "
+                           f"{fp16_k.shape[0]} rows of {fp16_k.shape[1]} tokens")
+
+
 def _kv_call(fn, a_k, b_k, s_k, a_v, b_v, s_v, fp16_k, batch_size, offset, width, page_size, cache_seqlens, block_table, wbits):
+    _check_kv_range(fp16_k, batch_size, offset, width, page_size)
     dim = fp16_k.shape[2] * fp16_k.shape[3]
     seq_stride = fp16_k.shape[1] * dim
     pages = 0
@@ -372,6 +383,7 @@ def q_to_fp16_kv(k_in, k_out, k_scales, v_in, v_out, v_scales, batch_size: int, 
     _dtype(k_in, torch.uint8, "k_in")
     _dtype(k_out, torch.float16, "k_out")
     _check_kv_shapes(k_out, k_in, v_out, v_in, wbits)
+    _check_kv_range(k_out, batch_size, offset, width, page_size)
     # C ABI order is (in, scales, out)
     dim = k_out.shape[2] * k_out.shape[3]
     seq_stride = k_out.shape[1] * dim

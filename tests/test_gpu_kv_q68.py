@@ -131,6 +131,42 @@ def test_kv_partial_range_leaves_rest_untouched(wbits):
         assert not (q[:, 5:8] == 0xAB).all() and not (s[:, 5:8] == 7.0).all()
 
 
+@pytest.mark.parametrize("wbits", [4, 6, 8])
+def test_kv_widening_stays_inside_the_tensor(wbits):
+    """A row of 2 * 64 values is a quarter of a 512-value block, so one token widens to four.  With one token per batch row
+    the widening must stop at the end of each row: every row is converted as itself, and the memory after the last row (two
+    guard rows of the same allocation here) is neither read into nor written.  A range outside the rows is refused."""
+    from exllamav2_b200 import ext as ext_c
+    from exllamav2_b200.ext import none_tensor
+    kb, vb = kv_q68.widths(wbits)
+    R = 6
+    big = torch.randn((R + 2, 1, 2, 64), dtype=torch.half, device=DEV)
+    kq, ks = _state(big.shape, kb, 0xAB)
+    vq, vs = _state(big.shape, vb, 0xAB)
+    ks.fill_(7.0)
+    vs.fill_(7.0)
+    ext_c.fp16_to_q_kv(big[:R], kq[:R], ks[:R], big[:R], vq[:R], vs[:R], R, 0, 1, 0, none_tensor, none_tensor, wbits)
+    torch.cuda.synchronize()
+    x = big[:R].cpu().numpy()
+    for q, s, bits in ((kq, ks, kb), (vq, vs, vb)):
+        assert (q[R:] == 0xAB).all() and (s[R:] == 7.0).all(), "wrote past the last row"
+        pq, ps = kv_q68.kv_pack(x.reshape(R, 1, -1), bits)
+        assert np.array_equal(cases.u16(s[:R].cpu().numpy().reshape(R, 1, -1)), cases.u16(ps))
+        assert _off_by_one_ok(q[:R].cpu().numpy().reshape(R, 1, -1), pq, bits)
+    out = torch.full((R + 2, 1, 2, 64), 3.0, dtype=torch.half, device=DEV)
+    out_v = out.clone()
+    ext_c.q_to_fp16_kv(kq[:R], out[:R], ks[:R], vq[:R], out_v[:R], vs[:R], R, 0, 1, 0, none_tensor, none_tensor, wbits)
+    torch.cuda.synchronize()
+    for o, q, s, bits in ((out, kq, ks, kb), (out_v, vq, vs, vb)):
+        assert (o[R:] == 3.0).all(), "wrote past the last row"
+        want = kv_q68.kv_unpack(q[:R].cpu().numpy().reshape(R, 1, -1), s[:R].cpu().numpy().reshape(R, 1, -1), bits)
+        assert np.array_equal(cases.u16(o[:R].cpu().numpy().reshape(R, 1, -1)), cases.u16(want))
+    with pytest.raises(RuntimeError, match="outside the tensor"):
+        ext_c.fp16_to_q_kv(big[:R], kq[:R], ks[:R], big[:R], vq[:R], vs[:R], R, 0, 2, 0, none_tensor, none_tensor, wbits)
+    with pytest.raises(RuntimeError, match="outside the tensor"):
+        ext_c.fp16_to_q_kv(big[:R], kq[:R], ks[:R], big[:R], vq[:R], vs[:R], R + 1, 0, 1, 0, none_tensor, none_tensor, wbits)
+
+
 def test_kv_rejects_bad_wbits_and_shapes():
     from exllamav2_b200 import ext as ext_c
     from exllamav2_b200.ext import none_tensor
