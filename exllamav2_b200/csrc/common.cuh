@@ -148,6 +148,16 @@ __device__ __forceinline__ uint32_t lds32(uint32_t addr) {
     asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
     return v;
 }
+__device__ __forceinline__ uint32_t lds_u16(uint32_t addr) {
+    unsigned short v;
+    asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ void stu128(uint32_t addr, uint4 v) {
+    asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+// orders this thread's earlier generic-proxy shared-memory accesses before later async-proxy (bulk copy) writes
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 #endif
 
 }  // namespace exl2b

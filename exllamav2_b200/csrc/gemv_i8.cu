@@ -25,7 +25,9 @@
 //     launch PLAN built on the host once per matrix structure (I8Plan below): the device walks 16-byte descriptors.
 //   * a warp streams its share of a block's bytes (layout.h: one contiguous stream per block) with cp.async.bulk into a
 //     private byte arena (a ring of variable-size stages placed by the host) and never synchronises with another warp in the
-//     main loop; per quantisation group one fp32 FMA with a scale read from the matrix' dense scale table (QMatrix::wtab).
+//     main loop; per quantisation group one fp32 FMA with a scale from the matrix' dense scale table (QMatrix::wtab).  The
+//     main loop issues no global load that it waits for: a group's scale row travels with the group's last stage (same bulk
+//     copy barrier) and the stage list is read from a shared-memory window that the stage copies refill ahead of use.
 //   * when the producer of the row scattered a copy in this matrix's stored-row order (I8Out::c_perm), the prologue reads the
 //     row with one 16-byte load per thread instead of eight 2-byte gathers.
 #include <string.h>
@@ -63,8 +65,16 @@ struct I8Mat {
 // A warp's weight arena is a byte ring (not fixed slots): the host places every stage, records after which stage's consumption its
 // space is free (that is the `request` count above), and the first stages -- everything that fits the arena, for small matrices the
 // warp's WHOLE share -- are requested before the dependency wait.  Stage s completes on mbarrier s % I8_BARS, parity (s / I8_BARS) & 1.
+// The same barrier covers two small copies that travel with stage s:
+//   * for a DF_FLUSH stage, the 32-column scale row of its group (64 B of fp16, or 128 B of GPTQ scale | zero << 16) into slot
+//     s % I8_BARS of the warp's scale ring.  At most I8_BARS stages are in flight, so stage s + I8_BARS (the next user of the
+//     slot) is requested only after stage s has been consumed.
+//   * descriptor s + I8_BARS into slot (s + I8_BARS) % I8_LWIN of the warp's list window.  Consuming stage s reads descriptor s
+//     and requests stages up to s + I8_BARS, all of which arrived with stages <= s; the slot it overwrites held descriptor
+//     s - I8_BARS, consumed before stage s could be requested.  Descriptors 0 .. I8_BARS - 1 are loaded before the first request.
 constexpr uint32_t DF_FLUSH = 1, DF_BLOCK_DONE = 2, DF_GPTQ = 4;
 constexpr int I8_BARS = 8;
+constexpr int I8_LWIN = 2 * I8_BARS;
 
 struct I8Params {
     I8Mat mat[I8_MAX_MATS];
@@ -80,9 +90,9 @@ struct I8Params {
     float norm_eps;
     int mode, x_permuted;
     int norm_permuted;                // norm_w is already in stored-row order (QMatrix::normp_buf)
-    int l1_hints;                     // descriptor loads L1::evict_last, scale loads L1::no_allocate
     int l2_prefetch;                  // prefetch the part of a warp's share that does not fit its arena into L2 before the wait
     int arena;                        // bytes of a warp's weight arena
+    int srow;                         // bytes of a scale ring slot: 64 (fp16 scale rows), 128 when a matrix is GPTQ
     int busy_ctas;                    // CTAs that own blocks; the rest of the grid only keeps its SM slot occupied (see the kernel)
     unsigned int* slot_cnt;           // CTAs of this launch that are done (self-resetting)
     unsigned long long* dbg;          // optional globaltimer stamps (exl2b_debug_set), NULL in production
@@ -92,16 +102,18 @@ struct I8Params {
 
 // dynamic shared-memory map of a CTA (byte offsets, every region 16-byte aligned) -- one definition for host and device
 struct I8Smem {
-    uint32_t act, asum, ascale, emit, total;
+    uint32_t act, asum, ascale, emit, scl, lst, total;
 };
-__host__ __device__ inline I8Smem i8_smem_map(int warps, int arena, int KS) {
+__host__ __device__ inline I8Smem i8_smem_map(int warps, int arena, int KS, int srow) {
     auto up = [](uint32_t x) { return (x + 15u) & ~15u; };
     I8Smem m;
     m.act = up((uint32_t)warps * (uint32_t)arena);                   // staged row: [KS][64 B]
     m.asum = up(m.act + (uint32_t)KS * 64u);                          // [KS] integer sum of a slab's row values
     m.ascale = up(m.asum + (uint32_t)KS * 4u);                        // [KS/4 + 1] scale of a 128-k block
     m.emit = up(m.ascale + (uint32_t)(KS / 4 + 1) * 4u);              // [warp][2][32] partial sums of split blocks
-    m.total = up(m.emit + (uint32_t)warps * 256u);
+    m.scl = up(m.emit + (uint32_t)warps * 256u);                      // [warp][I8_BARS][srow] scale rows of the flush stages in flight
+    m.lst = up(m.scl + (uint32_t)(warps * I8_BARS * srow));           // [warp][I8_LWIN] stage-list window (16-byte descriptors)
+    m.total = up(m.lst + (uint32_t)(warps * I8_LWIN * 16));
     return m;
 }
 
@@ -115,24 +127,6 @@ __device__ __forceinline__ int dp4a_uu(uint32_t a, uint32_t b, int c) {
     int d;
     asm("dp4a.u32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
     return d;
-}
-
-// descriptor / scale loads with L1 policies: the (small, re-read) stage lists are kept, the (read-once) scale entries pass through.
-// With 222 KB of the SM's 256 KB configured as shared memory the L1 is 28 KB for 32 warps.
-__device__ __forceinline__ uint4 ldg_keep(const uint4* p) {
-    uint4 v;
-    asm volatile("ld.global.nc.L1::evict_last.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
-    return v;
-}
-__device__ __forceinline__ uint32_t ldg_pass_u16(const void* p) {
-    unsigned short v;
-    asm volatile("ld.global.nc.L1::no_allocate.u16 %0, [%1];" : "=h"(v) : "l"(p));
-    return v;
-}
-__device__ __forceinline__ uint32_t ldg_pass_u32(const void* p) {
-    uint32_t v;
-    asm volatile("ld.global.nc.L1::no_allocate.u32 %0, [%1];" : "=r"(v) : "l"(p));
-    return v;
 }
 
 // ---- one slab (32 k) of the warp's 32-column block: integer dot products, one column per lane -------------------------------
@@ -357,7 +351,7 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
     }
 
     // ---- this CTA's blocks and this warp's stage list, straight from the host-built plan (nothing here depends on the
-    //      previous launch).  Descriptors are read through L1 where needed, one stage ahead of their use.
+    //      previous launch).
     const uint32_t cinfo = __ldg(P.plan_cta + blockIdx.x);
     const int blk0 = (int)(cinfo & 0xffffu), nb = (int)(cinfo >> 16);
     const uint32_t fw0 = __ldg(P.plan_first + blockIdx.x * I8_WARPS + warp), fw1 = __ldg(P.plan_first + blockIdx.x * I8_WARPS + warp + 1);
@@ -366,7 +360,7 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
     const uint4* const list = P.plan_desc + f0;
 
     // shared-memory map: generic pointers for the prologue's stores, 32-bit shared-space addresses (`lds*`) for the main loop
-    const I8Smem sm = i8_smem_map(I8_WARPS, P.arena, KS);
+    const I8Smem sm = i8_smem_map(I8_WARPS, P.arena, KS, P.srow);
     uint8_t* const act_g = smem + sm.act;
     int* const asum_s = reinterpret_cast<int*>(smem + sm.asum);
     float* const ascale_s = reinterpret_cast<float*>(smem + sm.ascale);
@@ -375,53 +369,41 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
     asm volatile("mov.u32 %0, %1;" : "=r"(sbase) : "r"(smem_addr(smem)));
     const uint32_t ring = sbase + (uint32_t)warp * (uint32_t)P.arena;
     const uint32_t act = sbase + sm.act, asum = sbase + sm.asum, ascale = sbase + sm.ascale;
+    const uint32_t sring = sbase + sm.scl + (uint32_t)(warp * I8_BARS * P.srow), lwin = sbase + sm.lst + (uint32_t)(warp * I8_LWIN * 16);
     uint32_t bar0;
     asm volatile("mov.u32 %0, %1;" : "=r"(bar0) : "r"(smem_addr(&bars[warp * I8_BARS])));
 
-    // per-matrix base pointers of the current matrix (a launch fuses up to 3; a warp changes matrix at most twice)
-    uint32_t mi_cur = 0u;
-    const uint8_t* pk_cur = P.mat[0].packed;
-    const uint8_t* wt_cur = reinterpret_cast<const uint8_t*>(P.mat[0].wtab);
-    auto select_mat = [&](uint32_t mi) {          // warp-uniform
-        if (mi != mi_cur) {
-            mi_cur = mi;
-            pk_cur = mi == 0 ? P.mat[0].packed : (mi == 1 ? P.mat[1].packed : P.mat[2].packed);
-            wt_cur = reinterpret_cast<const uint8_t*>(mi == 0 ? P.mat[0].wtab : (mi == 1 ? P.mat[1].wtab : P.mat[2].wtab));
-        }
-    };
     // request stages [s0, s0 + cnt) into their places in the arena: lane j decodes and issues stage s0 + j (cnt <= I8_BARS), so
-    // a batch of requests costs one descriptor decode, not one per stage.  `d` is lane j's descriptor (stage s0 + j), loaded by
-    // the caller well ahead of the request.
+    // a batch of requests costs one descriptor decode, not one per stage.  `d` is lane j's descriptor (stage s0 + j).  With the
+    // stage come its group's scale row (flush stages) and descriptor s + I8_BARS, on the same barrier (see DF_FLUSH above).
     auto issue_stages = [&](int s0, int cnt, uint4 d) {
         if (lane < cnt) {
             const int s = s0 + lane;
             const uint32_t mi = (d.z >> 22) & 3u;
             const uint8_t* pk = mi == 0 ? P.mat[0].packed : (mi == 1 ? P.mat[1].packed : P.mat[2].packed);
+            const uint8_t* wt = reinterpret_cast<const uint8_t*>(mi == 0 ? P.mat[0].wtab : (mi == 1 ? P.mat[1].wtab : P.mat[2].wtab));
             const uint32_t bytes = ((d.z >> 24) & 0xffu) << 7;
-            const uint32_t bar = bar0 + ((uint32_t)s & (I8_BARS - 1)) * 8u;
-            mbar_arrive_expect_tx(bar, bytes);
+            const uint32_t esz = (d.z & (DF_GPTQ << 18)) ? 4u : 2u;
+            const uint32_t sbytes = (d.z & (DF_FLUSH << 18)) ? 32u * esz : 0u;
+            const bool lnext = s + I8_BARS < nst;
+            const uint32_t slot = (uint32_t)s & (I8_BARS - 1);
+            const uint32_t bar = bar0 + slot * 8u;
+            mbar_arrive_expect_tx(bar, bytes + sbytes + (lnext ? 16u : 0u));
             bulk_copy_g2s(ring + ((d.w >> 16) & 0xffu) * 128u, pk + d.x, bytes, bar);
+            if (sbytes) bulk_copy_g2s(sring + slot * (uint32_t)P.srow, wt + (size_t)d.y * esz, sbytes, bar);
+            if (lnext) bulk_copy_g2s(lwin + ((uint32_t)(s + I8_BARS) & (I8_LWIN - 1)) * 16u, list + s + I8_BARS, 16u, bar);
         }
     };
-    auto load_req = [&](int s0) -> uint4 {          // lane j's descriptor of stage s0 + j (the next candidates for a request)
-        uint4 d = make_uint4(0u, 0u, 0u, 0u);
-        if (lane < I8_BARS && s0 + lane < nst) d = P.l1_hints ? ldg_keep(list + s0 + lane) : __ldg(list + s0 + lane);
-        return d;
-    };
-    // scale (and GPTQ zero point) of the group a stage belongs to, for this lane's column
-    auto fetch_scale = [&](uint4 d) -> uint32_t {
-        select_mat((d.z >> 22) & 3u);
-        const uint32_t idx = d.y + (uint32_t)lane;
-        if (P.l1_hints)
-            return (d.z & (DF_GPTQ << 18)) ? ldg_pass_u32(reinterpret_cast<const uint32_t*>(wt_cur) + idx)
-                                            : ldg_pass_u16(reinterpret_cast<const unsigned short*>(wt_cur) + idx);
-        return (d.z & (DF_GPTQ << 18)) ? __ldg(reinterpret_cast<const uint32_t*>(wt_cur) + idx)
-                                        : (uint32_t)__ldg(reinterpret_cast<const unsigned short*>(wt_cur) + idx);
-    };
-    uint4 dcur = make_uint4(0u, 0u, 0u, 0u);
-    if (nst > 0) dcur = P.l1_hints ? ldg_keep(list) : __ldg(list);
+    // descriptors 0 .. I8_BARS - 1 into the window; every later one arrives with the stage I8_BARS before it
+    uint4 dfirst = make_uint4(0u, 0u, 0u, 0u);
+    if (lane < I8_BARS && lane < nst) {
+        dfirst = __ldg(list + lane);
+        stu128(lwin + (uint32_t)lane * 16u, dfirst);
+    }
+    fence_proxy_async();                   // these window slots are later overwritten by bulk copies
+    __syncwarp();
     I8_STAMP(8);
-    issue_stages(0, n_pre, load_req(0));
+    issue_stages(0, n_pre, dfirst);
     int next_req = n_pre;
     // EXPERIMENT, off by default (EXL2B_I8_L2PF=1): pull the rest of the warp's share into L2 now (one bulk prefetch per stage),
     // while the previous launch is still computing.  Off because the 20-30 MB burst of the next launch competes with the
@@ -436,8 +418,6 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
                 bulk_prefetch_l2(pk + d.x, ((d.z >> 24) & 0xffu) << 7);
             }
         }
-    uint32_t wraw = 0u;
-    if (nst > 0) wraw = fetch_scale(dcur);
     I8_STAMP(9);
 
     // ---- static operands of the prologue, fetched before the dependency wait: permutation indices (when the row has to be
@@ -629,11 +609,10 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
     int S = 0, blk_slabs = 0, emits = 0;
 #pragma unroll 1
     for (int s = 0; s < nst; ++s) {
-        const uint4 d = dcur;
-        if (s + 1 < nst) dcur = P.l1_hints ? ldg_keep(list + s + 1) : __ldg(list + s + 1);      // next descriptor: in flight during this stage
+        const uint4 d = lds128(lwin + ((uint32_t)s & (I8_LWIN - 1)) * 16u);
         const int nreq = (int)((d.w >> 24) & 15u);
-        const uint4 dreq = load_req(next_req);                   // and the ones of the stages this stage's space will be given to
-        mbar_wait(bar0 + ((uint32_t)s & (I8_BARS - 1)) * 8u, ((uint32_t)s >> 3) & 1u);
+        const uint32_t slot8 = (uint32_t)s & (I8_BARS - 1);
+        mbar_wait(bar0 + slot8 * 8u, ((uint32_t)s >> 3) & 1u);
         const int ks = (int)(d.z & 0x7ffu), n = (int)((d.z >> 11) & 7u), bits = (int)((d.z >> 14) & 15u);
         const uint32_t slot = ring + ((d.w >> 16) & 0xffu) * 128u;
         const uint32_t xs = act + (uint32_t)ks * 64u, as = asum + (uint32_t)ks * 4u;
@@ -648,6 +627,14 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
             else if (opaque() == 8) S += consume_stage<8>(slot, n, xs, as, lane, am, ae);
             else S += consume_stage<2>(slot, n, xs, as, lane, am, ae);
         }
+        // what this stage's barrier delivered besides the weights: the descriptors of the stages its space will be given to,
+        // and (flush stages) this lane's scale -- read before the requests below may overwrite the scale slot
+        uint4 dreq = make_uint4(0u, 0u, 0u, 0u);
+        if (lane < nreq) dreq = lds128(lwin + ((uint32_t)(next_req + lane) & (I8_LWIN - 1)) * 16u);
+        uint32_t wraw = 0u;
+        if (d.z & (DF_FLUSH << 18))
+            wraw = (d.z & (DF_GPTQ << 18)) ? lds32(sring + slot8 * (uint32_t)P.srow + (uint32_t)lane * 4u)
+                                           : lds_u16(sring + slot8 * (uint32_t)P.srow + (uint32_t)lane * 2u);
         __syncwarp();
         {                                          // the space this stage occupied is free: request the stages waiting for it
             issue_stages(next_req, nreq, dreq);
@@ -664,7 +651,6 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
             am[0] = am[1] = am[2] = am[3] = 0;
             ae[0] = ae[1] = 0;
             S = 0;
-            if (s + 1 < nst) wraw = fetch_scale(dcur);      // scales of the next group
             if (d.z & (DF_BLOCK_DONE << 18)) {
                 const int blk = blk0 + (int)(d.w & 0xffffu);
                 if (blk_slabs == KS) {
@@ -799,7 +785,7 @@ struct I8Plan {
     uint32_t* d_first = nullptr;
     uint32_t* d_cta = nullptr;
     uint32_t* d_red = nullptr;
-    int ctas = 0, lcap = 0, arena = 0;
+    int ctas = 0, lcap = 0, arena = 0, srow = 64;
 };
 struct I8PlanMat {
     int N, KS, is_gptq, num_regions;
@@ -910,15 +896,9 @@ static void i8_build_lists(const I8PlanMat* mats, int nm, const unsigned short* 
     first.push_back((uint32_t)desc.size());
 }
 
-static int i8_get_plan(int device, const I8PlanMat* mats, int nm, int sms, int warps, I8Plan* out) {
-    std::string key((const char*)mats, sizeof(I8PlanMat) * nm);
-    const int extra[3] = {nm, sms, warps};
-    key.append((const char*)extra, sizeof(extra));
-    std::lock_guard<std::mutex> lk(g_plan_mutex);
-    auto it = g_plans[device].find(key);
-    if (it != g_plans[device].end()) { *out = it->second; return 0; }
-
-    I8Plan pl;
+// the host half of a plan: partition, arena size, scale-slot size and stage lists of one launch structure on `sms` CTAs
+static int i8_plan_host(const I8PlanMat* mats, int nm, int sms, int warps, I8Plan& pl, std::vector<uint4>& desc,
+                        std::vector<uint32_t>& first, std::vector<uint32_t>& cta, std::vector<uint32_t>& red) {
     std::vector<uint32_t> blk_bytes;
     for (int i = 0; i < nm; ++i) {
         // only blocks that hold real columns (the last strip of a padded matrix may contain all-padding blocks)
@@ -931,16 +911,33 @@ static int i8_get_plan(int device, const I8PlanMat* mats, int nm, int sms, int w
     // two launches co-resident per SM (227 KB, 1 KB reserved per CTA) is what lets the next launch prefetch: a CTA gets at most
     // 111 KB of dynamic shared memory (EXL2B_I8_SMEM overrides), and what the staged row / lists leave of it is split into the warps' weight arenas
     static const int smem_budget = [] { const char* e = getenv("EXL2B_I8_SMEM"); return e ? atoi(e) : 111 * 1024; }();
-    std::vector<uint4> desc;
-    std::vector<uint32_t> first, cta, red;
+    pl.srow = 64;
+    for (int i = 0; i < nm; ++i)
+        if (mats[i].is_gptq) pl.srow = 128;
     pl.arena = 8192;
     for (;;) {
         desc.clear(); first.clear(); cta.clear();
         i8_build_lists(mats, nm, cta_blk, pl.ctas, warps, pl.arena, desc, first, cta, red, &pl.lcap);
-        if ((int)i8_smem_map(warps, pl.arena, mats[0].KS).total <= smem_budget || pl.arena <= 2048) break;
+        if ((int)i8_smem_map(warps, pl.arena, mats[0].KS, pl.srow).total <= smem_budget || pl.arena <= 2048) break;
         pl.arena -= 128;
     }
     EXL2B_REQUIRE(desc.size() < (1u << 26), "too many stages");
+    return 0;
+}
+
+static int i8_get_plan(int device, const I8PlanMat* mats, int nm, int sms, int warps, I8Plan* out) {
+    std::string key((const char*)mats, sizeof(I8PlanMat) * nm);
+    const int extra[3] = {nm, sms, warps};
+    key.append((const char*)extra, sizeof(extra));
+    std::lock_guard<std::mutex> lk(g_plan_mutex);
+    auto it = g_plans[device].find(key);
+    if (it != g_plans[device].end()) { *out = it->second; return 0; }
+
+    I8Plan pl;
+    std::vector<uint4> desc;
+    std::vector<uint32_t> first, cta, red;
+    const int rc = i8_plan_host(mats, nm, sms, warps, pl, desc, first, cta, red);
+    if (rc) return rc;
     EXL2B_CUDA(cudaMalloc(&pl.d_desc, desc.size() * sizeof(uint4) + 16));
     EXL2B_CUDA(cudaMalloc(&pl.d_first, first.size() * 4));
     EXL2B_CUDA(cudaMalloc(&pl.d_cta, cta.size() * 4));
@@ -1004,6 +1001,9 @@ int gemv_i8_launch(int device, cudaStream_t stream, const I8Out* outs, int nm, c
         EXL2B_REQUIRE(v.KS == P.KS, "fused matrices must share K");
         EXL2B_REQUIRE((v.perm == nullptr) == (P.perm == nullptr), "fused matrices must share their row permutation");
         EXL2B_REQUIRE(q->wtab, "matrix has no scale table");
+        // scale rows are bulk-copied from (group * N + 32 * block) * (2 or 4) bytes: 16-byte aligned because N % 8 == 0, which
+        // exl2b_qmatrix_create requires (the reference's q_scale / qzeros pack 8 columns per word)
+        EXL2B_REQUIRE(v.N % 8 == 0, "width %d is not a multiple of 8", v.N);
         EXL2B_REQUIRE(q->packed_bytes < (1ull << 32), "matrix too large for 32-bit stage offsets");
         I8Mat& m = P.mat[i];
         m.packed = reinterpret_cast<const uint8_t*>(v.packed);
@@ -1039,12 +1039,11 @@ int gemv_i8_launch(int device, cudaStream_t stream, const I8Out* outs, int nm, c
     P.plan_cta = pl.d_cta;
     P.plan_red = pl.d_red;
     P.arena = pl.arena;
+    P.srow = pl.srow;
     P.busy_ctas = pl.ctas;
     static const int l2pf = [] { const char* e = getenv("EXL2B_I8_L2PF"); return e ? atoi(e) : 0; }();
     P.l2_prefetch = l2pf;
-    static const int l1h = [] { const char* e = getenv("EXL2B_I8_L1HINT"); return e ? atoi(e) : 0; }();
-    P.l1_hints = l1h;
-    const size_t smem_total = i8_smem_map(warps, P.arena, P.KS).total;
+    const size_t smem_total = i8_smem_map(warps, P.arena, P.KS, P.srow).total;
     EXL2B_REQUIRE(smem_total <= 200 * 1024, "shared memory budget exceeded (%zu bytes, K = %d)", smem_total, P.K);
     extern unsigned long long* g_dbg;
     extern int g_dbg_cta, g_dbg_slot;
@@ -1101,5 +1100,42 @@ extern "C" int exl2b_debug_plan(int N, int KS, int is_gptq, uint32_t blk_stream_
     memcpy(first, f.data(), f.size() * 4);
     if (red) memcpy(red, r.data(), r.size() * 4);          // [ceil(N / 32)]
     *n_desc = (int)d.size();
+    return 0;
+}
+
+// host-only diagnostics hook (tests/test_i8_smem_operands.py): the whole plan gemv_i8_launch would make for a launch of nm fused
+// matrices on `ctas` CTAs of `warps` warps.  mats: per matrix 5 + 5 * MAX_REGIONS ints (N, KS, is_gptq, blk_stream_bytes,
+// num_regions, then per region ks_begin, bits, spg_log2, group_base, off_base).  desc: capacity cap_desc x 4 words; first:
+// capacity cap_first words.  info: [0] CTAs with blocks, [1] descriptors, [2] arena bytes per warp, [3] scale-slot bytes,
+// [4] dynamic shared memory of a CTA, [5] longest stage list.
+extern "C" int exl2b_debug_i8_plan(const int* mats, int nm, int ctas, int warps, uint32_t* desc, int cap_desc, uint32_t* first,
+                                   int cap_first, int* info) {
+    EXL2B_REQUIRE(mats && desc && first && info, "null argument");
+    EXL2B_REQUIRE(nm >= 1 && nm <= exl2b::I8_MAX_MATS && ctas > 0 && ctas <= exl2b::I8_MAX_CTAS && warps > 0, "bad argument");
+    exl2b::I8PlanMat pm[exl2b::I8_MAX_MATS];
+    memset(pm, 0, sizeof(pm));
+    for (int i = 0; i < nm; ++i) {
+        const int* r = mats + i * (5 + 5 * exl2b::MAX_REGIONS);
+        EXL2B_REQUIRE(r[4] >= 1 && r[4] <= exl2b::MAX_REGIONS && r[1] == mats[1], "bad matrix %d", i);
+        pm[i].N = r[0]; pm[i].KS = r[1]; pm[i].is_gptq = r[2]; pm[i].blk_stream_bytes = (uint32_t)r[3]; pm[i].num_regions = r[4];
+        for (int g = 0; g < r[4]; ++g) {
+            const int* q = r + 5 + 5 * g;
+            pm[i].reg[g] = exl2b::QRegion{q[0], q[1], q[2], q[3], (uint32_t)q[4]};
+        }
+    }
+    exl2b::I8Plan pl;
+    std::vector<uint4> d;
+    std::vector<uint32_t> f, c, red;
+    const int rc = exl2b::i8_plan_host(pm, nm, ctas, warps, pl, d, f, c, red);
+    if (rc) return rc;
+    EXL2B_REQUIRE((int)d.size() <= cap_desc && (int)f.size() <= cap_first, "output buffers too small (%zu, %zu)", d.size(), f.size());
+    memcpy(desc, d.data(), d.size() * sizeof(uint4));
+    memcpy(first, f.data(), f.size() * 4);
+    info[0] = pl.ctas;
+    info[1] = (int)d.size();
+    info[2] = pl.arena;
+    info[3] = pl.srow;
+    info[4] = (int)exl2b::i8_smem_map(warps, pl.arena, pm[0].KS, pl.srow).total;
+    info[5] = pl.lcap;
     return 0;
 }

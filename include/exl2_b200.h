@@ -176,6 +176,11 @@ int exl2b_debug_set_records(unsigned long long* records);
 int exl2b_debug_plan(int N, int KS, int is_gptq, uint32_t blk_stream_bytes, const int* regions, int num_regions, int ctas, int warps,
                      int slot_bytes, uint32_t* desc, int cap_desc, uint32_t* first, int* ctas_used, int* n_desc, int* lcap,
                      uint32_t* red);
+/* host-only: the whole batch-1 GEMV plan of a launch of nm fused matrices (arena, scale-slot size, shared memory, stage lists);
+ * mats holds 5 + 5 * 6 ints per matrix: N, KS, is_gptq, blk_stream_bytes, num_regions, then (ks_begin, bits, spg_log2,
+ * group_base, off_base) per region.  info: CTAs, descriptors, arena bytes, scale-slot bytes, shared-memory bytes, longest list. */
+int exl2b_debug_i8_plan(const int* mats, int nm, int ctas, int warps, uint32_t* desc, int cap_desc, uint32_t* first, int cap_first,
+                        int* info);
 
 /* Stand-in for flash_attn_with_kvcache (third-party in the reference, attn.py:602-613): appends the q_len new K/V rows
  * to the paged fp16 cache at [seqlen, seqlen+q_len) and attends causally.  q [batch,q_len,H,hd], k/v_new
