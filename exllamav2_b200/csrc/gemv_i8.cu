@@ -1068,6 +1068,8 @@ int gemv_i8_launch(int device, cudaStream_t stream, const I8Out* outs, int nm, c
 
 }  // namespace exl2b
 
+extern "C" int exl2b_row_gemv_i8(void) { return exl2b::gemv_i8_enabled() ? 1 : 0; }
+
 // host-only diagnostics hook (tests/test_i8_emulation.py): the block -> CTA partition gemv_i8_launch would use
 extern "C" int exl2b_debug_partition(const uint32_t* block_bytes, int num_blocks, int ctas, uint16_t* out, int* used) {
     EXL2B_REQUIRE(block_bytes && out && used && num_blocks > 0 && ctas > 0 && ctas <= exl2b::I8_MAX_CTAS, "bad argument");

@@ -64,6 +64,7 @@ def _sig(name, restype, *argtypes):
 _sig("exl2b_last_error", c_char_p)
 _sig("exl2b_version", c_int)
 _sig("exl2b_launch_count", c_uint64)
+_sig("exl2b_row_gemv_i8", c_int)
 _sig("exl2b_qmatrix_create", c_int, POINTER(_QMatrixDesc), c_void_p, POINTER(c_void_p))
 _sig("exl2b_qmatrix_destroy", c_int, c_void_p)
 _sig("exl2b_qmatrix_info", c_int, c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_uint64))
@@ -138,6 +139,11 @@ def _stream(t: torch.Tensor):
 
 def launch_count() -> int:
     return int(lib.exl2b_launch_count())
+
+
+def row_gemv_i8() -> bool:
+    """True if single rows run on the integer GEMV (csrc/gemv_i8.cu), False if on the wgmma kernel (EXL2B_GEMV=tc at load)."""
+    return bool(lib.exl2b_row_gemv_i8())
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -268,12 +268,17 @@ class ExLlamaV2Decoder:
         self.fused_attn = os.environ.get("EXL2B_REF_KV_SEQUENCE") is None
         # producer epilogues feed consumer activation buffers (needs the default LAYOUT_TC matrix layout)
         self.chained = os.environ.get("EXL2B_NO_CHAIN") is None
-        # single rows (bs = 1 decode) run on the HBM-bound integer GEMV (csrc/gemv_i8.cu) in the reference's own op sequence
-        self.row_gemv = os.environ.get("EXL2B_GEMV", "")[:1] != "t"
         for L in self.layers:
             L.chain_attn = ext_c.make_chain([L.q_proj.q_handle, L.k_proj.q_handle, L.v_proj.q_handle], L.input_norm)
             L.chain_mlp = ext_c.make_chain([L.gate.q_handle, L.up.q_handle], L.post_norm)
         self.chain_head = ext_c.make_chain([self.lm_head.q_handle], self.final_norm)
+
+    @property
+    def row_gemv(self) -> bool:
+        """Single rows (bs = 1 decode) run on the HBM-bound integer GEMV (csrc/gemv_i8.cu), unless the library was loaded with
+        EXL2B_GEMV=tc.  Read from the library, not settable here: a chained single-row launch leaves the head's input in the
+        format of the library's path, and a head picked for the other path would read it as garbage."""
+        return ext_c.row_gemv_i8()
 
     # -- one decoder step over `q_len` new tokens per sequence (q_len small; rows = B * q_len) --
     def _forward_tokens(self, x, q, k, v, attn_out, q_len: int):

@@ -32,6 +32,10 @@ const char* exl2b_last_error(void);
 int exl2b_version(void);
 /* Number of kernels this library has launched since load (bench.py reports it as gpu_launches). */
 uint64_t exl2b_launch_count(void);
+/* 1 if single rows run on the integer GEMV (the default), 0 if on the wgmma kernel (EXL2B_GEMV=tc, read once at load).  A
+ * chained single-row producer writes its consumer's input in the format of this path, so host code that picks the consumer
+ * (the decode head) must follow it. */
+int exl2b_row_gemv_i8(void);
 
 /* ---- QMatrix ------------------------------------------------------------------------------------------------
  * replaces make_q_matrix (ext_qmatrix.cpp:21-111) / QMatrix::QMatrix (cuda/q_matrix.cu:49-196).

@@ -226,6 +226,76 @@ def test_prefill_2048_rows_llama_shape():
     lin.unload()
 
 
+# ---- many rows over more than one column window: gemm_big dequantises at most BIG_TEMP_BYTES of columns at a time ----------
+
+BIG_TEMP_BYTES = 64 << 20       # csrc/gemm_big.cu
+STRIP_N = 128                   # columns per strip of the default (tensor-core) layout, csrc/layout.h strip_n
+WINDOW_CASES = {                # dequantised 4096 x N fp16 > 64 MB, last strip ragged
+    "exl2_54": dict(K=4096, N=8224, bits=(5, 4), bits_prop=(0.1, 0.9), group_size=128, seed=201, bias=True),
+    "gptq_act": dict(K=4096, N=8200, group_size=128, seed=202, act_order=True, bias=True),
+}
+_WINDOW_W = {}
+
+
+def _windows(K, N):
+    """(windows, columns of the last window) of gemm_big_launch for a K x N matrix."""
+    per_window = max(1, BIG_TEMP_BYTES // (K * STRIP_N * 2))
+    strips = -(-N // STRIP_N)
+    n = -(-strips // per_window)
+    return n, N - (n - 1) * per_window * STRIP_N
+
+
+def _window_case(name):
+    """(checkpoint tensors incl. bias, oracle W) -- bias is drawn last, so the weights are the same with and without it."""
+    import synth
+    if name not in _WINDOW_W:
+        kw = WINDOW_CASES[name]
+        w_np = synth.make_exl2(**kw) if "bits" in kw else synth.make_gptq(**kw)
+        W = oracle.exl2_reconstruct(w_np) if "bits" in kw else oracle.gptq_reconstruct(w_np)
+        _WINDOW_W[name] = (w_np, W)
+    return _WINDOW_W[name]
+
+
+@pytest.mark.parametrize("M", [17, 40, 300])
+@pytest.mark.parametrize("mode", ["clear", "accumulate"])
+@pytest.mark.parametrize("bias", [False, True], ids=["nobias", "bias"])
+@pytest.mark.parametrize("name", list(WINDOW_CASES))
+def test_gemm_many_rows_multi_window(name, bias, mode, M):
+    """Every column window after the first (strip0 > 0), the ragged last window, bias and accumulate per window, into a strided
+    c whose padding must stay zero -- against fp64 a @ W_oracle."""
+    from exllamav2_b200 import ext as ext_c
+    from exllamav2_b200.linear import ExLlamaV2Linear, load_tensor_dict
+    K, N = WINDOW_CASES[name]["K"], WINDOW_CASES[name]["N"]
+    windows, last = _windows(K, N)
+    assert windows == 2 and 0 < last < STRIP_N, (windows, last)
+    w_full, W = _window_case(name)
+    w_np = {k: v for k, v in w_full.items() if bias or k != "bias"}
+    lin = ExLlamaV2Linear(K, N, has_bias=bias, key=name, device=DEV)
+    lin.load(load_tensor_dict(w_np, DEV))
+    rng = np.random.default_rng(M + 7 * bias)
+    a = rng.normal(0, 1, size=(M, K)).astype(np.float16)
+    c0 = rng.normal(0, 1, size=(M, N)).astype(np.float16)
+    a_buf = torch.zeros((M, K + 8), dtype=torch.half, device=DEV)
+    a_buf[:, :K] = torch.from_numpy(a).to(DEV)
+    c_buf = torch.zeros((M, N + 24), dtype=torch.half, device=DEV)
+    c_buf[:, :N] = torch.from_numpy(c0).to(DEV)         # clear: must be overwritten, not added to
+    if mode == "clear":
+        ext_c.gemm_half_q_half(a_buf[:, :K], lin.q_handle, c_buf[:, :N], False)
+    else:
+        ext_c.gemm_half_q_half_accum(a_buf[:, :K], lin.q_handle, c_buf[:, :N])
+    truth = oracle.gemm_truth(a, W, w_np.get("bias"), c0 if mode == "accumulate" else None)
+    got = c_buf[:, :N].cpu().numpy()
+    err = oracle.rel_l2(got, truth)
+    assert err <= GEMM_TOL, f"{name} bias={bias} {mode} M={M}: rel_l2 {err:.2e}"
+    # every window on its own (a wrong window offset leaves the overall error small when the window is narrow)
+    c1 = N - last
+    err_last = oracle.rel_l2(got[:, c1:], truth[:, c1:])
+    assert err_last <= GEMM_TOL, f"last window ({last} columns): rel_l2 {err_last:.2e}"
+    assert oracle.rel_l2(got[:, :c1], truth[:, :c1]) <= GEMM_TOL
+    assert torch.count_nonzero(c_buf[:, N:]).item() == 0
+    lin.unload()
+
+
 def test_two_streams_do_not_share_scratch():
     """Calls on different streams of one device run concurrently and must not share scratch (SURVEY.md 8b: re-entrant per handle):
     every row regime (1 row: integer GEMV, 4 rows: wgmma kernel, 40 rows: dense path), two matrices, two streams, many
