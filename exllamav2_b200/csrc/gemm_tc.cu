@@ -816,8 +816,11 @@ int gemm_tc_launch(int device, cudaStream_t stream, GemvMat* mats, int nm, int M
     // stage = the largest group of any matrix of the launch, per 32-column block
     int stage_bytes = 0;
     for (int i = 0; i < nm; ++i)
-        for (int r = 0; r < mats[i].w.num_regions; ++r)
+        for (int r = 0; r < mats[i].w.num_regions; ++r) {
+            // a stage's activations are one TC_ACT_STAGE (128 k): a larger group would overrun the activation ring
+            EXL2B_REQUIRE(mats[i].w.reg[r].spg_log2 <= 2, "quantisation groups above 128 rows are not supported by the wgmma kernel");
             stage_bytes = std::max(stage_bytes, (1 << mats[i].w.reg[r].spg_log2) * block_bytes(mats[i].w.reg[r].bits));
+        }
     EXL2B_REQUIRE(stage_bytes > 0 && stage_bytes <= 4096, "quantisation groups above 128 rows are not supported by the wgmma kernel");
     P.tc_stage_bytes = stage_bytes;
     const int header = ((TC_SMEM_BARS + TC_SMEM_MISC + 2 * GEMV_MTOK * 128 * 4 + GEMV_MTOK * 128 * 2 + 128 + TC_CORR_FLOATS * 4 + 1023) / 1024) * 1024;

@@ -76,17 +76,25 @@ int gemv_launch(int device, cudaStream_t stream, GemvMat* mats, int nm, int M, c
     return gemm_tc_launch(device, stream, mats, nm, M, norm_w, norm_eps, epilogue, ex);
 }
 
-// The wgmma kernel stages one quantisation group of a 32-column block per ring slot (<= 4 KB): groups of 256+ rows above 4
-// bits, or ungrouped GPTQ, do not fit.  Such matrices take the dense path for every row count above one.
+// The wgmma kernel stages one quantisation group of a 32-column block per ring slot: at most 4 slabs (128 rows, the size of
+// its activation stage) and 4 KB of weights.  Groups of 256+ rows (EXL2 g256+, GPTQ g256+, ungrouped GPTQ) do not fit; such
+// matrices take the dense path for every row count above one.
 bool gemm_tc_supported(const QMatView& v) {
     for (int r = 0; r < v.num_regions; ++r)
-        if ((1 << v.reg[r].spg_log2) * block_bytes(v.reg[r].bits) > 4096) return false;
+        if (v.reg[r].spg_log2 > 2 || (1 << v.reg[r].spg_log2) * block_bytes(v.reg[r].bits) > 4096) return false;
     return true;
 }
 
 }  // namespace exl2b
 
 using namespace exl2b;
+
+extern "C" int exl2b_qmatrix_tc_supported(exl2b_qmatrix_t h, int* supported) {
+    const QMatrix* q = (const QMatrix*)h;
+    EXL2B_REQUIRE(q && supported, "null argument");
+    *supported = q->v.layout == LAYOUT_TC && gemm_tc_supported(q->v) ? 1 : 0;
+    return 0;
+}
 
 extern "C" int exl2b_gemm_half_q_half(exl2b_qmatrix_t h, const uint16_t* a, int lda, uint16_t* c, int ldc, int m,
                                       int clear, int force_cuda, exl2b_stream_t stream) {

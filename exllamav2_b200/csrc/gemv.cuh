@@ -92,5 +92,7 @@ int gemm_big_launch(const QMatrix* q, const half* a, int lda, half* c, int ldc, 
 
 // can `ex` be honoured for these matrices / this row count?  (LAYOUT_TC, one pass)
 bool gemv_supports_extras(const GemvMat* mats, int nm, int M);
+// can the wgmma kernel stage the matrix's quantisation groups (<= 4 KB per 32-column block)?
+bool gemm_tc_supported(const QMatView& v);
 
 }  // namespace exl2b

@@ -68,6 +68,7 @@ _sig("exl2b_row_gemv_i8", c_int)
 _sig("exl2b_qmatrix_create", c_int, POINTER(_QMatrixDesc), c_void_p, POINTER(c_void_p))
 _sig("exl2b_qmatrix_destroy", c_int, c_void_p)
 _sig("exl2b_qmatrix_info", c_int, c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_uint64))
+_sig("exl2b_qmatrix_tc_supported", c_int, c_void_p, POINTER(c_int))
 _sig("exl2b_reconstruct", c_int, c_void_p, c_void_p, c_void_p)
 _sig("exl2b_gemm_half_q_half", c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p)
 _sig("exl2b_gemm_half_q_half_norm", c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_int, c_void_p)
@@ -210,6 +211,14 @@ def q_matrix_info(handle: int) -> dict:
     h, w, g, gq, pb = c_int(), c_int(), c_int(), c_int(), c_uint64()
     _check(lib.exl2b_qmatrix_info(handle, ctypes.byref(h), ctypes.byref(w), ctypes.byref(g), ctypes.byref(gq), ctypes.byref(pb)))
     return {"height": h.value, "width": w.value, "groups": g.value, "is_gptq": bool(gq.value), "packed_bytes": pb.value}
+
+
+def qmatrix_tc_supported(handle: int) -> bool:
+    """True if the 2..16-row kernel can stage this matrix's quantisation groups, so chained launches above one row can use it
+    (include/exl2_b200.h exl2b_qmatrix_tc_supported).  Otherwise the blocks run it on the dense path above one row."""
+    s = c_int()
+    _check(lib.exl2b_qmatrix_tc_supported(handle, ctypes.byref(s)))
+    return bool(s.value)
 
 
 def reconstruct(q_handle: int, output: torch.Tensor):

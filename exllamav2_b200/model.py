@@ -272,6 +272,16 @@ class ExLlamaV2Decoder:
             L.chain_attn = ext_c.make_chain([L.q_proj.q_handle, L.k_proj.q_handle, L.v_proj.q_handle], L.input_norm)
             L.chain_mlp = ext_c.make_chain([L.gate.q_handle, L.up.q_handle], L.post_norm)
         self.chain_head = ext_c.make_chain([self.lm_head.q_handle], self.final_norm)
+        # above one row a chained step runs every matrix on the wgmma kernel, which cannot stage groups of 256+ rows (EXL2 or GPTQ
+        # g256+, ungrouped GPTQ; include/exl2_b200.h exl2b_qmatrix_tc_supported)
+        self.tc_staged = all(ext_c.qmatrix_tc_supported(l.q_handle) for l in self.linears)
+
+    def _chains(self, rows: int) -> bool:
+        """Does a step of `rows` rows (batch x new tokens) run the chained schedule?  One row on the integer GEMV always can;
+        more rows only when every matrix can be staged by the wgmma kernel (otherwise the blocks take the dense path)."""
+        if not (self.chained and self.fused_attn and rows <= 8):
+            return False
+        return self.tc_staged or (rows == 1 and self.row_gemv)
 
     @property
     def row_gemv(self) -> bool:
@@ -286,7 +296,7 @@ class ExLlamaV2Decoder:
         B = self.batch_size
         stream = torch.cuda.current_stream(self.device).cuda_stream
         H, KVH, hd = cfg.num_heads, cfg.num_kv_heads, cfg.head_dim
-        if self.chained and self.fused_attn and B * q_len <= 8:
+        if self._chains(B * q_len):
             return self._forward_tokens_chained(x, q, k, v, attn_out, q_len)
         for li, L in enumerate(self.layers):
             if self.fused_attn and q_len <= 8:
@@ -346,7 +356,7 @@ class ExLlamaV2Decoder:
             self._forward_tokens_chained(self.x, self.q, self.k, self.v, self.attn_out, 1, head=True)
             ext_c.gemv_norm(self.x.view(1, -1), self.lm_head.q_handle, self.final_norm, self.cfg.norm_eps, self.logits, prepared=True)
             return
-        if self.chained and self.fused_attn and self.batch_size <= 8:
+        if self._chains(self.batch_size):
             self._forward_tokens_chained(self.x, self.q, self.k, self.v, self.attn_out, 1, head=True)
             ext_c.gemm_half_q_half_prepared(self.lm_head.q_handle, self.logits, True, self.cfg.norm_eps)
             return

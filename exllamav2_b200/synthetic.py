@@ -73,9 +73,11 @@ def random_gptq(K: int, N: int, group_size: int = 128, device="cuda:0", seed: in
                 weight_std: float | None = None, perm_seed: int | None = None) -> dict:
     """Random GPTQ 4-bit tensors.  weight_std: standard deviation of the dequantised weights (std of q - zero for uniform
     nibbles is ~6.5); None: scales ~ U(0.002, 0.02) as in SURVEY.md 8d C1.  perm_seed: matrices quantised against the same
-    input share their act-order g_idx."""
+    input share their act-order g_idx.  group_size <= 0: ungrouped (GPTQ's group_size -1), one group and g_idx all zero."""
     gen = torch.Generator(device=device)
     gen.manual_seed(seed)
+    if group_size <= 0:
+        group_size = K
     G = K // group_size
     g_idx = (torch.arange(K) // group_size).to(torch.int32)
     if act_order:

@@ -68,6 +68,10 @@ typedef struct exl2b_qmatrix_desc {
 int exl2b_qmatrix_create(const exl2b_qmatrix_desc* desc, exl2b_stream_t stream, exl2b_qmatrix_t* out);
 int exl2b_qmatrix_destroy(exl2b_qmatrix_t h);                     /* free_q_matrix, ext_qmatrix.cpp:187-194 */
 int exl2b_qmatrix_info(exl2b_qmatrix_t h, int* height, int* width, int* groups, int* is_gptq, uint64_t* packed_bytes);
+/* *supported = 1 if the 2..16-row kernel (and with it every chained launch above one row) can run this matrix: it stages one
+ * quantisation group of a 32-column block at a time, at most 128 rows (4 KB at 8 bits).  Matrices with larger groups (EXL2 or
+ * GPTQ g256+, ungrouped GPTQ) take the dense path at every row count above one instead, and cannot be chained there. */
+int exl2b_qmatrix_tc_supported(exl2b_qmatrix_t h, int* supported);
 
 /* reconstruct (ext_qmatrix.cpp:196-210, QMatrix::reconstruct q_matrix.cu:499-553):
  * out fp16[K, N] row-major in ORIGINAL row order, out[perm[k'], n] = half(q - zero) * half(scale), bit-exact. */

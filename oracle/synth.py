@@ -89,8 +89,11 @@ def make_exl2(K: int, N: int, bits=(4,), bits_prop=(1.0,), group_size=128, seed:
 
 def make_gptq(K: int, N: int, group_size: int = 128, seed: int = 0, act_order: bool = False, bias: bool = False) -> dict:
     """Synthetic GPTQ 4-bit linear (SURVEY.md 8d C1): uniform random nibbles, scales ~ U(0.002, 0.02),
-    g_idx = arange//g, or a seeded permutation of it for act-order."""
+    g_idx = arange//g, or a seeded permutation of it for act-order.  group_size <= 0: ungrouped (GPTQ's group_size -1),
+    one group over all K rows and g_idx all zero -- with or without act-order, as such checkpoints ship."""
     rng = np.random.default_rng(seed)
+    if group_size <= 0:
+        group_size = K
     assert K % group_size == 0 and N % 8 == 0 and K % 8 == 0
     G = K // group_size
     q = rng.integers(0, 16, size=(K, N), dtype=np.int64)

@@ -17,8 +17,10 @@ Every decode and prompt schedule the decoder has is run here, on a page table th
   L   prefill_rows of 252 tokens, then D1 steps across position 256 (the second page)
 
 Models: test-small (MHA, hd 64, 512-wide kv row), test-tiny (GQA, hd 64, 128-wide kv row: fused schedules only -- the reference
-sequence re-quantises neighbouring tokens there, a documented divergence), a 2-layer hd-128 GQA model and a GPTQ act-order plan
-on test-small's dimensions; K/V cache Q4 / Q6 / Q8.
+sequence re-quantises neighbouring tokens there, a documented divergence), a 2-layer hd-128 GQA model and, on test-small's
+dimensions, a GPTQ g128 act-order plan, an all-8-bit g128 EXL2 plan (groups exactly at the wgmma kernel's 4 KB stage) and an
+ungrouped act-order GPTQ plan (groups it cannot stage: above one row its steps take the fused, un-chained branch); K/V cache
+Q4 / Q6 / Q8.
 
 Per call: (1) logits (decode) or the returned hidden state (prompt) per sequence vs the fp64 truth, rel-L2 below a measured
 bound per schedule (DESIGN.md §3.6), scaled up only on inputs whose fp16 floor is atypically large (see FLOOR_TYPICAL);
@@ -68,6 +70,12 @@ def _cfg(model):
     if model == "gptq":
         return LlamaConfig("test-small-gptq", 512, 1408, 8, 8, 64, 2, 512, max_seq_len=512,
                            plan=QuantPlan(attn=("gptq", 128, True), mlp=[("gptq", 128, True)], head=((6,), (1.0,), 128)))
+    if model == "exl2-8bpw":     # every linear 8-bit g128, head included: groups exactly at the wgmma kernel's 4 KB stage
+        b8 = ((8,), (1.0,), 128)
+        return LlamaConfig("test-small-8bpw", 512, 1408, 8, 8, 64, 2, 512, max_seq_len=512, plan=QuantPlan(attn=b8, mlp=[b8], head=b8))
+    if model == "gptq-nogroup":  # ungrouped act-order GPTQ (group_size -1): groups the wgmma kernel cannot stage
+        return LlamaConfig("test-small-gptq-nogroup", 512, 1408, 8, 8, 64, 2, 512, max_seq_len=512,
+                           plan=QuantPlan(attn=("gptq", -1, True), mlp=[("gptq", -1, True)], head=((6,), (1.0,), 128)))
     raise KeyError(model)
 
 
@@ -242,8 +250,13 @@ def _names(calls):
 
 def _check_branch(sched, kind, calls, dec, L):
     """Assert the host branch a call took, from the entry points it reached."""
-    from exllamav2_b200 import model
+    from exllamav2_b200 import ext, model
     B = dec.batch_size
+    # above one row the chained schedule runs every matrix on the wgmma kernel: a model with a matrix it cannot stage takes the
+    # fused, un-chained branch there instead (D5 as D3 / D6, P1 through q_attn_forward_1)
+    staged = all(ext.qmatrix_tc_supported(l.q_handle) for l in dec.linears)
+    if not staged and sched == "D5":
+        sched = "D6"
     names = _names(calls)
     attn1 = _named(calls, "q_attn_forward_1")
     attn1_ex = _named(calls, "q_attn_forward_1_ex")
@@ -265,10 +278,10 @@ def _check_branch(sched, kind, calls, dec, L):
             assert len(fused) == L and all(kw.get("rope") is None for _, kw in fused)
             assert head == {"gemm_half_q_half_prepared"}
         elif sched in ("D3", "D6"):
-            assert dec.fused_attn and not (dec.chained and B <= 8)
+            assert dec.fused_attn and not (dec.chained and B <= 8 and staged)
             assert not attn1_ex and rows1 == [B] and len(fused) == L and len(_named(calls, "q_mlp_forward_")) == L
             assert head == {"gemm_half_q_half"} and "rms_norm" in names
-            if sched == "D6":
+            if sched == "D6" and staged:
                 assert 8 < B <= 16          # the 9..16-row wgmma, not the many-row path
         elif sched == "D4":
             assert not dec.fused_attn and not fused and len(ref_attn) == L
@@ -281,7 +294,11 @@ def _check_branch(sched, kind, calls, dec, L):
         qlens = [a[3] for a, _ in attn1_ex] + [a[3] for a, _ in attn1]
         if sched == "P1":
             assert dec.chained and dec.fused_attn and B == 1
-            assert not attn1 and [a[3] for a, _ in attn1_ex] == [8] * L + [3] * L
+            if staged:
+                assert not attn1 and [a[3] for a, _ in attn1_ex] == [8] * L + [3] * L
+            else:
+                assert not attn1_ex and [a[3] for a, _ in attn1] == [8] * L + [3] * L
+                assert [a[0].shape[1] for a, _ in fused] == [8] * L + [3] * L
             assert "gemv_norm" not in names and "gemm_half_q_half_prepared" not in names
         elif sched == "P2":
             assert dec.fused_attn and B == 3
@@ -386,6 +403,7 @@ DECODE_CASES = [
     ("D4", "small", 4), ("D4", "small", 6), ("D4", "small", 8), ("D4", "hd128", 4), ("D4", "gptq", 4),
     ("D5", "small", 4), ("D5", "tiny", 4), ("D5", "hd128", 8), ("D5", "gptq", 4),
     ("D6", "small", 4), ("D6", "tiny", 6), ("D6", "hd128", 4), ("D6", "gptq", 8),
+    ("D1", "exl2-8bpw", 4), ("D1", "gptq-nogroup", 8), ("D5", "exl2-8bpw", 6), ("D5", "gptq-nogroup", 4),
 ]
 
 
@@ -462,6 +480,9 @@ PROMPT_CASES = [
     ("P3c", "small", 4), ("P3c", "small", 8), ("P3c", "hd128", 6),
     ("P3a-sdpa", "small", 4), ("P3a-sdpa", "hd128", 8), ("P3b-sdpa", "small", 6), ("P3b-sdpa", "gptq", 4),
     ("P4", "small", 4), ("P4", "small", 6), ("P4", "small", 8), ("P4", "hd128", 4), ("P4", "gptq", 4),
+    ("P1", "exl2-8bpw", 4), ("P1", "gptq-nogroup", 6), ("P2", "exl2-8bpw", 8), ("P2", "gptq-nogroup", 4),
+    ("P3a", "exl2-8bpw", 6), ("P3a", "gptq-nogroup", 4), ("P3b", "gptq-nogroup", 8), ("P3c", "exl2-8bpw", 4),
+    ("P3c", "gptq-nogroup", 6),
 ]
 
 
