@@ -83,8 +83,63 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 
 int device_sm_count(int device);
 
+// ---- slot holders -----------------------------------------------------------------------------------------------
+// A launch whose grid has more CTAs than it has work for pads the grid to one CTA per SM: CTAs with blockIdx.x >= busy
+// hold their SM slot (slot_hold) until every working CTA has left (slot_release), so that no SM runs two CTAs of one launch
+// while another runs none (gemv_i8.cu).  The counter resets itself when the last CTA of the grid leaves.  Each kernel keeps
+// a ring of 127 such counters per device, so a counter is reused only after 127 launches of that kernel.
+struct SlotCounters {
+    unsigned int* dev[64] = {};
+    std::atomic<unsigned> seq{0};
+};
+inline int next_slot_counter(SlotCounters& s, int device, unsigned int** cnt) {
+    if (!s.dev[device]) {
+        EXL2B_CUDA(cudaMalloc(&s.dev[device], 128 * sizeof(unsigned int)));
+        EXL2B_CUDA(cudaMemset(s.dev[device], 0, 128 * sizeof(unsigned int)));
+    }
+    *cnt = s.dev[device] + (s.seq.fetch_add(1) % 127u);
+    return 0;
+}
+
 // ---- device-side PTX wrappers -----------------------------------------------------------------------------------
 #if defined(__CUDACC__)
+
+// one thread per CTA: count this CTA out of the launch
+__device__ __forceinline__ void slot_release(unsigned int* cnt) {
+    if (atomicAdd(cnt, 1u) == gridDim.x - 1u) *reinterpret_cast<volatile unsigned int*>(cnt) = 0u;
+}
+// one thread of a slot-holder CTA: wait for the `busy` working CTAs, then leave with them
+__device__ __forceinline__ void slot_hold(unsigned int* cnt, int busy) {
+    while (*reinterpret_cast<volatile unsigned int*>(cnt) < (unsigned)busy) __nanosleep(200);
+    slot_release(cnt);
+}
+
+__device__ __forceinline__ unsigned long long globaltimer() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+// optional phase stamps of a kernel whose params carry `dbg` / `dbg_cta` (exl2b_debug_set): stamp i of thread 0 of CTA dbg_cta;
+// stamp 0 also lowers dbg[6] to the earliest start over the grid (the kernel raises dbg[7] to the latest end itself)
+#define EXL2B_STAMP(P, i)                                                                                   \
+    do {                                                                                                    \
+        if ((P).dbg) {                                                                                      \
+            if (blockIdx.x == (P).dbg_cta && threadIdx.x == 0) (P).dbg[i] = exl2b::globaltimer();         \
+            if ((i) == 0 && threadIdx.x == 0) atomicMin((P).dbg + 6, exl2b::globaltimer());                \
+        }                                                                                                   \
+    } while (0)
+
+// integer dot product of four byte pairs plus c.  a: 4 unsigned bytes; b: 4 signed (us) or unsigned (uu) bytes
+__device__ __forceinline__ int dp4a_us(uint32_t a, uint32_t b, int c) {
+    int d;
+    asm("dp4a.u32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
+    return d;
+}
+__device__ __forceinline__ int dp4a_uu(uint32_t a, uint32_t b, int c) {
+    int d;
+    asm("dp4a.u32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
+    return d;
+}
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 

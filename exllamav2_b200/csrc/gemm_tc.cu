@@ -116,12 +116,6 @@ __device__ __forceinline__ half tc_gelu_h(half x) {
     return __float2half_rn(xf);
 }
 
-__device__ __forceinline__ unsigned long long tc_gtimer() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    return t;
-}
-#define TC_STAMP(i) do { if (P.dbg) { if (blockIdx.x == P.dbg_cta && tid == 0) P.dbg[i] = tc_gtimer(); if ((i) == 0 && tid == 0) atomicMin(P.dbg + 6, tc_gtimer()); } } while (0)
 
 template <int BITS>
 __device__ __forceinline__ void tc_load_words(const uint8_t* base, int lane, uint32_t* mw, uint32_t* ew) {
@@ -240,7 +234,7 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_kernel(const __grid_con
     const int wq = warp & 3, tidw = tid & 127;                      // warp in the WG; thread = weight column during the unpack
 
     griddep_launch_dependents();
-    TC_STAMP(0);
+    EXL2B_STAMP(P, 0);
 
     // shared memory: [barriers][misc][WG totals][fp16 tile][ssq][S1/S0] | [2 activation rings] | [2 x 2 A tiles] | [8 weight rings]
     const uint32_t smem0 = smem_addr(smem);
@@ -371,14 +365,14 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_kernel(const __grid_con
             setup_done = true;
             __syncthreads();
         }
-        TC_STAMP(1);
+        EXL2B_STAMP(P, 1);
 
         // everything above depended only on the weights; from here on the previous kernel's output is needed
         if (!waited) {
             griddep_wait();
             waited = true;
             after_wait();
-            TC_STAMP(2);
+            EXL2B_STAMP(P, 2);
         }
         if (wq == 0) {            // the activations of the groups primed above (same walk, scratch cursor)
             int t_ks = my0, t_r = c_r, t_spg = c_spg, t_end = c_end;
@@ -530,7 +524,7 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_kernel(const __grid_con
             waited = true;
             after_wait();
         }
-        TC_STAMP(4);
+        EXL2B_STAMP(P, 4);
 
         // the finishing CTA's scatter needs, per consumer, this column's destination row and RMSNorm weight: request them now, so
         // that the loads ride under the combine / split-K hand-off below instead of sitting on the tail of the launch
@@ -723,11 +717,11 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_kernel(const __grid_con
             }
         }
         __syncthreads();
-        TC_STAMP(5);
+        EXL2B_STAMP(P, 5);
         u += seg;
     }
 
-    if (P.dbg && tid == 0) atomicMax(P.dbg + 7, tc_gtimer());
+    if (P.dbg && tid == 0) atomicMax(P.dbg + 7, globaltimer());
 }
 
 // ---- host launcher -----------------------------------------------------------------------------------------------------

@@ -117,18 +117,6 @@ __host__ __device__ inline I8Smem i8_smem_map(int warps, int arena, int KS, int 
     return m;
 }
 
-// ---- small device helpers ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int dp4a_us(uint32_t a, uint32_t b, int c) {      // a: 4 unsigned bytes, b: 4 signed bytes
-    int d;
-    asm("dp4a.u32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
-    return d;
-}
-__device__ __forceinline__ int dp4a_uu(uint32_t a, uint32_t b, int c) {
-    int d;
-    asm("dp4a.u32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
-    return d;
-}
-
 // ---- one slab (32 k) of the warp's 32-column block: integer dot products, one column per lane -------------------------------
 // Staged row of a slab (64 B): XH[2j] / XH[2j+1] = high bytes of k = 8j + {0,4,1,5} / 8j + {2,6,3,7}; XL the low bytes.
 // That is the byte order every plane's masked words have (layout.h pair_word / pair_slot): (w & 0x0f0f0f0f) / (w & 0xf0f0f0f0)
@@ -312,15 +300,9 @@ __device__ __forceinline__ half gelu_h(half x) {        // cuda/q_mlp_activation
     return __float2half_rn(xf);
 }
 
-__device__ __forceinline__ unsigned long long i8_gtimer() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
 // stamps of thread 0 of CTA dbg_cta: 0 start, 1 first stages requested, 2 dependency wait over, 3 row staged,
 // 4 warp 0's main loop done, 5 all warps done, (6 = earliest CTA start, 7 = latest CTA end over the grid), 8 stage list in
-// shared memory, 9 first stages and scales requested
-#define I8_STAMP(i) do { if (P.dbg) { if (blockIdx.x == P.dbg_cta && tid == 0) P.dbg[i] = i8_gtimer(); if ((i) == 0 && tid == 0) atomicMin(P.dbg + 6, i8_gtimer()); } } while (0)
+// shared memory, 9 first stages and scales requested (EXL2B_STAMP)
 
 // ---- the kernel -----------------------------------------------------------------------------------------------------------
 template <int I8_WARPS>
@@ -332,8 +314,8 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int KS = P.KS;
-    I8_STAMP(0);
-    if (P.dbg_rec && tid == 0 && blockIdx.x < 160) P.dbg_rec[blockIdx.x * 4] = i8_gtimer();
+    EXL2B_STAMP(P, 0);
+    if (P.dbg_rec && tid == 0 && blockIdx.x < 160) P.dbg_rec[blockIdx.x * 4] = globaltimer();
     if (tid < I8_WARPS * I8_BARS) mbar_init(smem_addr(&bars[tid]), 1);
     mbar_fence_init();
     __syncthreads();
@@ -343,10 +325,7 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
     //      ONE CTA of every launch of the chain: an SM that has none would offer two free slots to the next launch, which then
     //      runs two of its CTAs there at half speed each while another SM idles.  So CTAs without blocks stay resident until the CTAs with blocks are done, then leave with them.
     if ((int)blockIdx.x >= P.busy_ctas) {
-        if (tid == 0) {
-            while (*reinterpret_cast<volatile unsigned int*>(P.slot_cnt) < (unsigned)P.busy_ctas) __nanosleep(200);
-            if (atomicAdd(P.slot_cnt, 1u) == gridDim.x - 1u) *reinterpret_cast<volatile unsigned int*>(P.slot_cnt) = 0u;
-        }
+        if (tid == 0) slot_hold(P.slot_cnt, P.busy_ctas);
         return;
     }
 
@@ -402,7 +381,7 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
     }
     fence_proxy_async();                   // these window slots are later overwritten by bulk copies
     __syncwarp();
-    I8_STAMP(8);
+    EXL2B_STAMP(P, 8);
     issue_stages(0, n_pre, dfirst);
     int next_req = n_pre;
     // EXPERIMENT, off by default (EXL2B_I8_L2PF=1): pull the rest of the warp's share into L2 now (one bulk prefetch per stage),
@@ -418,7 +397,7 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
                 bulk_prefetch_l2(pk + d.x, ((d.z >> 24) & 0xffu) << 7);
             }
         }
-    I8_STAMP(9);
+    EXL2B_STAMP(P, 9);
 
     // ---- static operands of the prologue, fetched before the dependency wait: permutation indices (when the row has to be
     //      gathered, or the norm weight has) and the norm weight of this thread's first octets
@@ -446,10 +425,10 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
         }
     }
 
-    I8_STAMP(1);
+    EXL2B_STAMP(P, 1);
     griddep_wait();                        // everything below may read what the previous launch wrote
-    I8_STAMP(2);
-    if (P.dbg_rec && tid == 0 && blockIdx.x < 160) P.dbg_rec[blockIdx.x * 4 + 1] = i8_gtimer();
+    EXL2B_STAMP(P, 2);
+    if (P.dbg_rec && tid == 0 && blockIdx.x < 160) P.dbg_rec[blockIdx.x * 4 + 1] = globaltimer();
 
     // ---- prologue: the row -> (optional RMSNorm weight / act*mul) -> 16-bit integers per 128-k block -> shared memory.
     //      Every CTA stages the whole row (its blocks span all of K); 1/rms is applied to the finished fp32 sums.
@@ -585,7 +564,7 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
         if (lane == 0) s_red[warp] = sumsq;
     }
     __syncthreads();
-    I8_STAMP(3);
+    EXL2B_STAMP(P, 3);
     float rrms = 1.f;
     if (P.mode == I8_RMSNORM) {
         float t = 0.f;
@@ -665,9 +644,9 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
             }
         }
     }
-    I8_STAMP(4);
+    EXL2B_STAMP(P, 4);
     __syncthreads();
-    I8_STAMP(5);
+    EXL2B_STAMP(P, 5);
 
     // ---- split-K never left the CTA: sum the warps' partials of each block in warp order (the plan says which warps hold them),
     //      finalise.  Blocks covered by one warp alone were finalised in the main loop (no partials).
@@ -683,12 +662,12 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
         }
         finalize_block(P, blk0 + b, lane, (b == warp) ? opre0 : out_pre(P, blk0 + b, lane), v * rrms);
     }
-    if (tid == 0 && atomicAdd(P.slot_cnt, 1u) == gridDim.x - 1u) *reinterpret_cast<volatile unsigned int*>(P.slot_cnt) = 0u;
-    if (P.dbg && lane == 0) atomicMax(P.dbg + 7, i8_gtimer());
+    if (tid == 0) slot_release(P.slot_cnt);
+    if (P.dbg && lane == 0) atomicMax(P.dbg + 7, globaltimer());
     if (P.dbg_rec && tid == 0 && blockIdx.x < 160) {
         unsigned smid;
         asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-        P.dbg_rec[blockIdx.x * 4 + 2] = i8_gtimer();
+        P.dbg_rec[blockIdx.x * 4 + 2] = globaltimer();
         P.dbg_rec[blockIdx.x * 4 + 3] = smid;
     }
 }
@@ -1052,13 +1031,9 @@ int gemv_i8_launch(int device, cudaStream_t stream, const I8Out* outs, int nm, c
     extern unsigned long long* g_dbg_rec;
     P.dbg_rec = (g_dbg_rec && P.dbg) ? g_dbg_rec + (size_t)((g_dbg_slot - 1) % 64) * 160 * 4 : nullptr;      // [64][160][4], CTAs 0..159
     // one CTA per SM, always (slot holders, see the kernel); a self-resetting counter per launch in flight
-    static unsigned int* slot_cnts[64] = {nullptr};
-    static std::atomic<unsigned> launch_seq{0};
-    if (!slot_cnts[device]) {
-        EXL2B_CUDA(cudaMalloc(&slot_cnts[device], 128 * sizeof(unsigned int)));
-        EXL2B_CUDA(cudaMemset(slot_cnts[device], 0, 128 * sizeof(unsigned int)));
-    }
-    P.slot_cnt = slot_cnts[device] + (launch_seq.fetch_add(1) % 127u);
+    static SlotCounters slot_cnts;
+    rc = next_slot_counter(slot_cnts, device, &P.slot_cnt);
+    if (rc) return rc;
     const int C = slot_holders_disabled() ? pl.ctas : std::max(pl.ctas, grid_ctas);
     if (warps == 16) EXL2B_CUDA(launch_pdl_f("i8", gemv_i8_kernel<16>, dim3(C), dim3(16 * 32), smem_total, stream, P));
     else if (warps == 12) EXL2B_CUDA(launch_pdl_f("i8", gemv_i8_kernel<12>, dim3(C), dim3(12 * 32), smem_total, stream, P));

@@ -1,10 +1,7 @@
 // Q4 / Q6 / Q8 K/V cache pack / unpack (exllamav2_ext/cuda/cache_q.cuh, cuda/cache.cu:143-497).
 //
 // Same arithmetic as the reference, op for op (so results are bit-identical to it on the same inputs):
-//   pack:   warp butterfly Hadamard-32 on two interleaved 32-vectors (unnormalised, fp16 adds), absmax over 32
-//           consecutive values, then
-//             4 bits: w = w / absmax * 8 + 8,     q = clamp(rn(w), 0, 15),  scale = absmax / 8    (two values per byte)
-//             8 bits: w = w / absmax * 128 + 128, q = clamp(rn(w), 0, 255), scale = absmax / 128  (one byte per value)
+//   pack:   Hadamard-32 and quantisation as kv_format.cuh defines them (the op order is stated there)
 //   unpack: (q - 8) * scale (or (q - 128) * scale) -> Hadamard -> * 1/32
 // wbits = 4: keys and values in 4 bits; 6: keys in 8 bits, values in 4 bits; 8: both in 8 bits (cache.cu:250-276).
 // What differs is the mapping to the machine: the reference runs 256-thread CTAs over 512-value blocks staged
@@ -14,95 +11,35 @@
 // over (k|v, sequence, token range) and the grid is sized to the actual work.
 #include <algorithm>
 
-#include "common.cuh"
+#include "kv_format.cuh"
 
 namespace exl2b {
 
-__device__ __forceinline__ half2 hadamard32(half2 w2, int lane) {
+// one warp: 64 fp16 values at `in` -> 64 * BITS / 8 packed bytes at `out`, 2 scales at `scales` (cache_q.cuh:78-108)
+template <int BITS>
+__device__ __forceinline__ void pack_unit(const half* __restrict__ in, uint8_t* __restrict__ out, half* __restrict__ scales,
+                                          int lane) {
+    constexpr int LPW = 16 / BITS;      // lanes per 32-bit output word
+    const KvCodes c = kv_quantise<BITS>(hadamard32_h(reinterpret_cast<const half2*>(in)[lane], lane));
+    uint32_t q = c.q0 | (c.q1 << BITS);
 #pragma unroll
-    for (int i = 1; i < 32; i <<= 1) {
-        const half2 pw2 = __shfl_xor_sync(0xffffffffu, w2, i);
-        uint32_t* w2i = reinterpret_cast<uint32_t*>(&w2);
-        const int32_t sfm = -static_cast<int32_t>(lane & i) >> 31;
-        *w2i ^= (sfm & 0x80008000);
-        w2 = __hadd2(w2, pw2);
-    }
-    return w2;
+    for (int s = 1; s < LPW; s <<= 1) q |= (__shfl_down_sync(0xffffffffu, q, s) << (2 * BITS * s));
+    if ((lane & (LPW - 1)) == 0) reinterpret_cast<uint32_t*>(out)[lane / LPW] = q;
+    if ((lane & 15) == 0) scales[lane >> 4] = c.scale;
 }
 
-// one warp: 64 fp16 values at `in` -> 32 packed bytes at `out`, 2 scales at `scales`
-__device__ __forceinline__ void pack_unit_q4(const half* __restrict__ in, uint8_t* __restrict__ out,
-                                             half* __restrict__ scales, int lane) {
-    half2 w2 = reinterpret_cast<const half2*>(in)[lane];
-    w2 = hadamard32(w2, lane);
-    half2 absmax2 = __habs2(w2);
-    half absmax = __hmax(__low2half(absmax2), __high2half(absmax2));
-    absmax = __hmax(absmax, __shfl_xor_sync(0xffffffffu, absmax, 8));
-    absmax = __hmax(absmax, __shfl_xor_sync(0xffffffffu, absmax, 4));
-    absmax = __hmax(absmax, __shfl_xor_sync(0xffffffffu, absmax, 2));
-    absmax = __hmax(absmax, __shfl_xor_sync(0xffffffffu, absmax, 1));
-    absmax2 = __half2half2(absmax);
-    const half2 c_8 = __half2half2(__float2half_rn(8));
-    const half c_i = __float2half_rn(1.0f / 8.0f);
-    w2 = __h2div(w2, absmax2);
-    w2 = __hfma2(w2, c_8, c_8);
-    const int q0 = min(max(__half2int_rn(__low2half(w2)), 0), 15);
-    const int q1 = min(max(__half2int_rn(__high2half(w2)), 0), 15);
-    uint32_t q = q0 | (q1 << 4);
-    q |= (__shfl_down_sync(0xffffffffu, q, 1) << 8);
-    q |= (__shfl_down_sync(0xffffffffu, q, 2) << 16);
-    if ((lane & 3) == 0) reinterpret_cast<uint32_t*>(out)[lane >> 2] = q;
-    if ((lane & 15) == 0) scales[lane >> 4] = __hmul(absmax, c_i);
-}
-
-__device__ __forceinline__ void unpack_unit_q4(const uint8_t* __restrict__ in, const half* __restrict__ scales,
-                                               half* __restrict__ out, int lane) {
+template <int BITS>
+__device__ __forceinline__ void unpack_unit(const uint8_t* __restrict__ in, const half* __restrict__ scales,
+                                            half* __restrict__ out, int lane) {
+    constexpr int LPW = 16 / BITS, MASK = (1 << BITS) - 1, ZERO = 1 << (BITS - 1);
     const half scale = __ldg(scales + (lane >> 4));
-    const uint32_t q = __ldg(reinterpret_cast<const uint32_t*>(in) + (lane >> 2));
-    const int shift0 = (lane & 3) * 8;
-    const int q0 = ((int)((q >> shift0) & 0x0f)) - 8;
-    const int q1 = ((int)((q >> (shift0 + 4)) & 0x0f)) - 8;
+    const uint32_t q = __ldg(reinterpret_cast<const uint32_t*>(in) + lane / LPW);
+    const int shift0 = (lane & (LPW - 1)) * 2 * BITS;
+    const int q0 = ((int)((q >> shift0) & MASK)) - ZERO;
+    const int q1 = ((int)((q >> (shift0 + BITS)) & MASK)) - ZERO;
     half2 w2 = __halves2half2(__int2half_rn(q0), __int2half_rn(q1));
     w2 = __hmul2(w2, __half2half2(scale));
-    w2 = hadamard32(w2, lane);
-    w2 = __hmul2(w2, __float2half2_rn(1.0f / 32.0f));
-    __stcg(reinterpret_cast<half2*>(out) + lane, w2);
-}
-
-// one warp: 64 fp16 values at `in` -> 64 bytes at `out` (value e at byte e), 2 scales at `scales` (cache_q.cuh:78-108)
-__device__ __forceinline__ void pack_unit_q8(const half* __restrict__ in, uint8_t* __restrict__ out,
-                                             half* __restrict__ scales, int lane) {
-    half2 w2 = reinterpret_cast<const half2*>(in)[lane];
-    w2 = hadamard32(w2, lane);
-    half2 absmax2 = __habs2(w2);
-    half absmax = __hmax(__low2half(absmax2), __high2half(absmax2));
-    absmax = __hmax(absmax, __shfl_xor_sync(0xffffffffu, absmax, 8));
-    absmax = __hmax(absmax, __shfl_xor_sync(0xffffffffu, absmax, 4));
-    absmax = __hmax(absmax, __shfl_xor_sync(0xffffffffu, absmax, 2));
-    absmax = __hmax(absmax, __shfl_xor_sync(0xffffffffu, absmax, 1));
-    absmax2 = __half2half2(absmax);
-    const half2 c_128 = __half2half2(__float2half_rn(128));
-    const half c_i = __float2half_rn(1.0f / 128.0f);
-    w2 = __h2div(w2, absmax2);
-    w2 = __hfma2(w2, c_128, c_128);
-    const int q0 = min(max(__half2int_rn(__low2half(w2)), 0), 255);
-    const int q1 = min(max(__half2int_rn(__high2half(w2)), 0), 255);
-    uint32_t q = q0 | (q1 << 8);
-    q |= (__shfl_down_sync(0xffffffffu, q, 1) << 16);
-    if ((lane & 1) == 0) reinterpret_cast<uint32_t*>(out)[lane >> 1] = q;
-    if ((lane & 15) == 0) scales[lane >> 4] = __hmul(absmax, c_i);
-}
-
-__device__ __forceinline__ void unpack_unit_q8(const uint8_t* __restrict__ in, const half* __restrict__ scales,
-                                               half* __restrict__ out, int lane) {
-    const half scale = __ldg(scales + (lane >> 4));
-    const uint32_t q = __ldg(reinterpret_cast<const uint32_t*>(in) + (lane >> 1));
-    const int shift0 = (lane & 1) * 16;
-    const int q0 = ((int)((q >> shift0) & 0xff)) - 128;
-    const int q1 = ((int)((q >> (shift0 + 8)) & 0xff)) - 128;
-    half2 w2 = __halves2half2(__int2half_rn(q0), __int2half_rn(q1));
-    w2 = __hmul2(w2, __half2half2(scale));
-    w2 = hadamard32(w2, lane);
+    w2 = hadamard32_h(w2, lane);
     w2 = __hmul2(w2, __float2half2_rn(1.0f / 32.0f));
     __stcg(reinterpret_cast<half2*>(out) + lane, w2);
 }
@@ -166,11 +103,11 @@ __global__ void __launch_bounds__(256) kv_q_kernel(const __grid_constant__ KvJob
         void* s = kv ? J.v_s : J.k_s;
         const bool q8 = (kv ? J.v_bits : J.k_bits) == 8;      // warp-uniform
         if (J.pack) {
-            if (q8) pack_unit_q8((const half*)a + el, (uint8_t*)b + el, (half*)s + el / 32, lane);
-            else pack_unit_q4((const half*)a + el, (uint8_t*)b + el / 2, (half*)s + el / 32, lane);
+            if (q8) pack_unit<8>((const half*)a + el, (uint8_t*)b + el, (half*)s + el / 32, lane);
+            else pack_unit<4>((const half*)a + el, (uint8_t*)b + el / 2, (half*)s + el / 32, lane);
         } else {
-            if (q8) unpack_unit_q8((const uint8_t*)a + el, (const half*)s + el / 32, (half*)b + el, lane);
-            else unpack_unit_q4((const uint8_t*)a + el / 2, (const half*)s + el / 32, (half*)b + el, lane);
+            if (q8) unpack_unit<8>((const uint8_t*)a + el, (const half*)s + el / 32, (half*)b + el, lane);
+            else unpack_unit<4>((const uint8_t*)a + el / 2, (const half*)s + el / 32, (half*)b + el, lane);
         }
     }
 }

@@ -90,8 +90,6 @@ _sig("exl2b_qmlp_create", c_int, POINTER(_QMlpDesc), POINTER(c_void_p))
 _sig("exl2b_qmlp_destroy", c_int, c_void_p)
 _sig("exl2b_qmlp_forward", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p)
 _sig("exl2b_qmlp_forward_gateup", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p)
-_sig("exl2b_paged_attn_decode_q4", c_int, *([c_void_p] * 10 + [c_int] * 7 + [c_float, c_void_p, c_void_p]))
-_sig("exl2b_paged_attn_decode_q4_ex", c_int, *([c_void_p] * 10 + [c_int] * 7 + [c_float, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]))
 _sig("exl2b_paged_attn_decode_q", c_int, *([c_void_p] * 10 + [c_int] * 7 + [c_float, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]))
 _sig("exl2b_paged_attn_status", c_int, c_int, POINTER(c_int))
 _sig("exl2b_paged_attn_clear_status", c_int, c_int)
