@@ -18,6 +18,8 @@
 // One CTA per (head, sequence); decode regime (q_len <= 8).  The kernel runs as phases over a per-CTA context (AttnCta):
 // prologue and staging, new-row quantisation and query rotation, scores, softmax, P V, append, end of the query.
 #include <algorithm>
+#include <map>
+#include <mutex>
 
 #include "gemv_i8.cuh"
 #include "kv_format.cuh"
@@ -804,6 +806,54 @@ using namespace exl2b;
 
 static int32_t* g_attn_err[64] = {nullptr};
 
+// Split-KV partial results and arrival counters, one set per (device, stream) like the wgmma workspace (gemv.cu): launches on
+// different streams never merge each other's partials.  Allocated once at the bound every split launch fits in and never
+// freed or moved, because a captured graph keeps the pointers it was captured with.  attn_launch_plan splits only when
+// H * B <= SMs (by_sms >= 2) and takes nsplit <= 2 * SMs / (H * B), so B * H * nsplit <= 2 * SMs: at most 2 * SMs * (128 + 2)
+// floats and SMs counters (tests/test_scratch_bound.py).  Created on first use: never inside a stream capture.
+struct AttnScratch {
+    float* ws = nullptr;
+    unsigned int* cnt = nullptr;
+    size_t ws_floats = 0, n_cnt = 0;
+};
+static std::map<std::pair<int, cudaStream_t>, AttnScratch> g_attn_scratch;
+static std::mutex g_attn_scratch_mutex;
+
+static int attn_scratch(int device, cudaStream_t stream, int sms, AttnScratch** out) {
+    std::lock_guard<std::mutex> lock(g_attn_scratch_mutex);
+    AttnScratch& s = g_attn_scratch[{device, stream}];
+    if (!s.ws) {
+        const size_t floats = (size_t)2 * sms * (128 + 2), cnt = (size_t)sms;
+        EXL2B_CUDA(cudaMalloc(&s.ws, floats * sizeof(float)));
+        EXL2B_CUDA(cudaMalloc(&s.cnt, cnt * sizeof(unsigned int)));
+        EXL2B_CUDA(cudaMemset(s.cnt, 0, cnt * sizeof(unsigned int)));
+        EXL2B_CUDA(cudaDeviceSynchronize());
+        s.ws_floats = floats;
+        s.n_cnt = cnt;
+    }
+    *out = &s;
+    return 0;
+}
+
+// exl2b_debug_scratch, attention kinds: the workspace or counters of (device, stream), NULL / 0 before their first use
+namespace exl2b {
+int attn_scratch_query(int device, cudaStream_t stream, int kind, void** ptr, size_t* bytes) {
+    std::lock_guard<std::mutex> lock(g_attn_scratch_mutex);
+    const auto it = g_attn_scratch.find({device, stream});
+    *ptr = nullptr;
+    *bytes = 0;
+    if (it == g_attn_scratch.end()) return 0;
+    if (kind == EXL2B_SCRATCH_ATTN_WS) {
+        *ptr = it->second.ws;
+        *bytes = it->second.ws_floats * sizeof(float);
+    } else {
+        *ptr = it->second.cnt;
+        *bytes = it->second.n_cnt * sizeof(unsigned int);
+    }
+    return 0;
+}
+}  // namespace exl2b
+
 extern "C" int exl2b_paged_attn_status(int device, int* status) {
     EXL2B_REQUIRE(status && device >= 0 && device < 64, "bad argument");
     *status = 0;
@@ -885,24 +935,16 @@ extern "C" int exl2b_paged_attn_decode_q(const uint16_t* q, const uint16_t* k_ne
         EXL2B_CUDA(cudaMemset(g_attn_err[dev], 0, sizeof(int32_t)));
     }
     P.err = g_attn_err[dev];
-    static float* g_ws[64] = {nullptr};
-    static unsigned int* g_cnt[64] = {nullptr};
-    static size_t g_ws_floats[64] = {0}, g_cnt_n[64] = {0};
     if (L.nsplit > 1) {
+        AttnScratch* s = nullptr;
+        int rc = attn_scratch(dev, (cudaStream_t)stream, sms, &s);
+        if (rc) return rc;
         const size_t need = (size_t)batch * num_heads * L.nsplit * (head_dim + 2), need_c = (size_t)batch * num_heads;
-        if (g_ws_floats[dev] < need) {
-            if (g_ws[dev]) cudaFree(g_ws[dev]);
-            EXL2B_CUDA(cudaMalloc(&g_ws[dev], need * sizeof(float)));
-            g_ws_floats[dev] = need;
-        }
-        if (g_cnt_n[dev] < need_c) {
-            if (g_cnt[dev]) cudaFree(g_cnt[dev]);
-            EXL2B_CUDA(cudaMalloc(&g_cnt[dev], need_c * sizeof(unsigned)));
-            EXL2B_CUDA(cudaMemset(g_cnt[dev], 0, need_c * sizeof(unsigned)));
-            g_cnt_n[dev] = need_c;
-        }
-        P.ws = g_ws[dev];
-        P.cnt = g_cnt[dev];
+        EXL2B_REQUIRE(need <= s->ws_floats && need_c <= s->n_cnt,
+                      "split-KV launch needs %zu floats / %zu counters, above the per-stream bound %zu / %zu", need, need_c,
+                      s->ws_floats, s->n_cnt);
+        P.ws = s->ws;
+        P.cnt = s->cnt;
     }
     P.nsplit = L.nsplit;
     P.sc_len = L.sc_len;

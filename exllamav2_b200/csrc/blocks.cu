@@ -19,13 +19,23 @@ struct QAttn {
     exl2b_qattn_desc d;
     int device;
     bool i8_qkv;          // q/k/v share K and the row permutation: one gemv_i8 launch for a single row
+    half* norm_p;         // the layernorm in q/k/v's stored-row order, taken at creation (single-row launches), or NULL
 };
 struct QMlp {
     exl2b_qmlp_desc d;
     int device;
     bool i8_gu;           // same for gate/up
     half* up_scratch;     // single-row up projection when the caller passes no temp_b (reference: temp_b of make_q_mlp)
+    half* norm_p;         // the layernorm in gate/up's stored-row order, as QAttn::norm_p
 };
+
+// the handle's copy of its layernorm in the stored-row order of the single-row GEMV's matrices (none without a permutation)
+static int block_norm_copy(const QMatrix* q, const void* layernorm, bool i8, half** out) {
+    *out = nullptr;
+    if (!layernorm || !i8 || !q->v.perm) return 0;
+    EXL2B_CUDA(cudaSetDevice(q->device));
+    return permuted_norm_copy(q, (const half*)layernorm, out);
+}
 
 static GemvMat make_mat(const QMatrix* q, const half* x, int ldx, half* c, int ldc, int clear) {
     GemvMat m = {};
@@ -129,13 +139,22 @@ extern "C" int exl2b_qattn_create(const exl2b_qattn_desc* d, exl2b_qattn_t* out)
                   "projection widths do not match the head layout");
     EXL2B_REQUIRE(q->device == k->device && q->device == v->device && q->device == o->device, "handles on different devices");
     const QMatrix* qkv[3] = {q, k, v};
-    QAttn* a = new QAttn{*d, q->device, gemv_i8_fusable(qkv, 3)};
+    const bool i8 = gemv_i8_fusable(qkv, 3);
+    half* norm_p = nullptr;
+    int rc = block_norm_copy(q, d->layernorm, i8, &norm_p);
+    if (rc) return rc;
+    QAttn* a = new QAttn{*d, q->device, i8, norm_p};
     *out = (exl2b_qattn_t)a;
     return 0;
 }
 
 extern "C" int exl2b_qattn_destroy(exl2b_qattn_t h) {
-    delete (QAttn*)h;
+    QAttn* a = (QAttn*)h;
+    if (a && a->norm_p) {
+        cudaSetDevice(a->device);
+        cudaFree(a->norm_p);
+    }
+    delete a;
     return 0;
 }
 
@@ -160,7 +179,8 @@ extern "C" int exl2b_qattn_forward_1_ex(exl2b_qattn_t h, const uint16_t* x, int 
         // q_proj's stored-row order by the producer launch (I8Out::c_perm -> q_proj's row buffer).  RoPE as in the reference
         // (q_attn.cu:271-300) unless the caller passes no tables: exl2b_paged_attn_decode_q rotates q / k as it reads them.
         const I8Out o[3] = {{mq, (half*)q, 1}, {mk, (half*)k, 1}, {mv, (half*)v, 1}};
-        I8Input in = {(const half*)x, nullptr, (const half*)d.layernorm, d.norm_epsilon, d.layernorm ? I8_RMSNORM : I8_PLAIN, 0};
+        I8Input in = {(const half*)x, nullptr, (const half*)d.layernorm, d.norm_epsilon, d.layernorm ? I8_RMSNORM : I8_PLAIN, 0,
+                      a->norm_p};
         if (input_prepared) {
             EXL2B_REQUIRE(mq->xp_buf, "input_prepared set, but no chained producer has written q_proj's input row");
             in.x = mq->xp_buf;
@@ -283,16 +303,21 @@ extern "C" int exl2b_qmlp_create(const exl2b_qmlp_desc* d, exl2b_qmlp_t* out) {
                   "mlp intermediate size mismatch");
     EXL2B_REQUIRE(g->device == u->device && (!dn || g->device == dn->device), "handles on different devices");
     const QMatrix* gu[2] = {g, u};
-    QMlp* m = new QMlp{*d, g->device, gemv_i8_fusable(gu, 2), nullptr};
+    const bool i8 = gemv_i8_fusable(gu, 2);
+    half* norm_p = nullptr;
+    int rc = block_norm_copy(g, d->layernorm, i8, &norm_p);
+    if (rc) return rc;
+    QMlp* m = new QMlp{*d, g->device, i8, nullptr, norm_p};
     *out = (exl2b_qmlp_t)m;
     return 0;
 }
 
 extern "C" int exl2b_qmlp_destroy(exl2b_qmlp_t h) {
     QMlp* m = (QMlp*)h;
-    if (m && m->up_scratch) {
+    if (m && (m->up_scratch || m->norm_p)) {
         cudaSetDevice(m->device);
-        cudaFree(m->up_scratch);
+        if (m->up_scratch) cudaFree(m->up_scratch);
+        if (m->norm_p) cudaFree(m->norm_p);
     }
     delete m;
     return 0;
@@ -327,7 +352,8 @@ extern "C" int exl2b_qmlp_forward_ex(exl2b_qmlp_t h, uint16_t* x, int rows, uint
         o[0].c_perm = dn->xp_buf;
         o[1].c_perm = dn->xp_buf + dn->v.K;
         o[0].out_invperm = o[1].out_invperm = dn->invperm;
-        I8Input in1 = {(const half*)x, nullptr, (const half*)d.layernorm, d.norm_epsilon, d.layernorm ? I8_RMSNORM : I8_PLAIN, 0};
+        I8Input in1 = {(const half*)x, nullptr, (const half*)d.layernorm, d.norm_epsilon, d.layernorm ? I8_RMSNORM : I8_PLAIN, 0,
+                       m->norm_p};
         if (input_prepared) {
             EXL2B_REQUIRE(g->xp_buf, "input_prepared set, but no chained producer has written gate_proj's input row");
             in1.x = g->xp_buf;
@@ -390,7 +416,8 @@ extern "C" int exl2b_qmlp_forward_gateup(exl2b_qmlp_t h, const uint16_t* x, int 
         // decode row: gate|up as one integer-GEMV launch (RMSNorm in its prologue), then act(gate) * up on the rank's slice
         if (!m->up_scratch) EXL2B_CUDA(cudaMalloc(&m->up_scratch, (size_t)d.intermediate_size * sizeof(half)));
         const I8Out o[2] = {{g, (half*)temp_a, 1}, {u, m->up_scratch, 1}};
-        const I8Input in = {(const half*)x, nullptr, (const half*)d.layernorm, d.norm_epsilon, d.layernorm ? I8_RMSNORM : I8_PLAIN, 0};
+        const I8Input in = {(const half*)x, nullptr, (const half*)d.layernorm, d.norm_epsilon, d.layernorm ? I8_RMSNORM : I8_PLAIN, 0,
+                            m->norm_p};
         int rc = gemv_i8_launch(m->device, (cudaStream_t)stream_, o, 2, in);
         if (rc) return rc;
         return exl2b_act_mul(temp_a, (const uint16_t*)m->up_scratch, 1, d.intermediate_size, d.act_gelu, stream_);

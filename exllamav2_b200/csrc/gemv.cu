@@ -156,3 +156,23 @@ extern "C" int exl2b_debug_set_records(unsigned long long* records) {
     exl2b::g_dbg_rec = records;
     return 0;
 }
+
+namespace exl2b {
+int attn_scratch_query(int device, cudaStream_t stream, int kind, void** ptr, size_t* bytes);
+}
+extern "C" int exl2b_debug_scratch(int device, exl2b_stream_t stream, int kind, void** ptr, size_t* bytes) {
+    EXL2B_REQUIRE(ptr && bytes && device >= 0 && device < 64, "bad argument");
+    EXL2B_REQUIRE(kind >= EXL2B_SCRATCH_ATTN_WS && kind <= EXL2B_SCRATCH_TC_XP, "unknown scratch kind %d", kind);
+    if (kind == EXL2B_SCRATCH_ATTN_WS || kind == EXL2B_SCRATCH_ATTN_CNT)
+        return attn_scratch_query(device, (cudaStream_t)stream, kind, ptr, bytes);
+    std::lock_guard<std::mutex> lock(g_ws_mutex);
+    *ptr = nullptr;
+    *bytes = 0;
+    const auto it = g_tc_ws.find({device, (cudaStream_t)stream});
+    if (it == g_tc_ws.end()) return 0;
+    const TcWorkspace& d = it->second;
+    if (kind == EXL2B_SCRATCH_TC_WS) { *ptr = d.ws; *bytes = d.ws_bytes; }
+    if (kind == EXL2B_SCRATCH_TC_CNT) { *ptr = d.counters; *bytes = (size_t)d.n_counters * sizeof(unsigned int); }
+    if (kind == EXL2B_SCRATCH_TC_XP) { *ptr = d.xp; *bytes = d.xp_bytes; }
+    return 0;
+}

@@ -89,7 +89,7 @@ struct I8Params {
     const half* norm_w;
     float norm_eps;
     int mode, x_permuted;
-    int norm_permuted;                // norm_w is already in stored-row order (QMatrix::normp_buf)
+    int norm_permuted;                // norm_w is already in stored-row order (I8Input::norm_wp)
     int l2_prefetch;                  // prefetch the part of a warp's share that does not fit its arena into L2 before the wait
     int arena;                        // bytes of a warp's weight arena
     int srow;                         // bytes of a scale ring slot: 64 (fp16 scale rows), 128 when a matrix is GPTQ
@@ -731,25 +731,27 @@ void i8_partition_blocks(const std::vector<uint32_t>& bytes, int ctas, unsigned 
     *used = c;
 }
 
-// RMSNorm weight in a matrix' stored-row order, cached on the matrix (first use: one tiny gather kernel; never inside a capture)
+// RMSNorm weight in a matrix' stored-row order.  Only a block handle keeps such a copy, made when the handle is created (as
+// the reference's handles take their tensors at creation); a bare call gathers the weight in the kernel, so no copy can
+// outlive or lag behind the weight it was made from.
 __global__ void gather_rows_kernel(half* __restrict__ out, const half* __restrict__ w, const uint16_t* __restrict__ perm, int K) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < K) out[i] = w[perm[i]];
 }
-static std::mutex g_normp_mutex;
-static int i8_permuted_norm(QMatrix* q, const half* norm_w, cudaStream_t stream, const half** out) {
-    std::lock_guard<std::mutex> lk(g_normp_mutex);
-    if (q->normp_src != norm_w) {
-        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-        cudaStreamIsCapturing(stream, &cs);
-        if (cs != cudaStreamCaptureStatusNone) { *out = nullptr; return 0; }      // first seen inside a capture: gather in the kernel instead
-        if (!q->normp_buf) EXL2B_CUDA(cudaMalloc(&q->normp_buf, (size_t)q->v.K * sizeof(half)));
-        gather_rows_kernel<<<(q->v.K + 255) / 256, 256, 0, stream>>>(q->normp_buf, norm_w, q->v.perm, q->v.K);
-        g_launch_count++;
-        EXL2B_CUDA(cudaGetLastError());
-        q->normp_src = norm_w;
+int permuted_norm_copy(const QMatrix* q, const half* norm_w, half** out) {
+    *out = nullptr;
+    half* p = nullptr;
+    EXL2B_CUDA(cudaDeviceSynchronize());             // the weight may still be in flight on any stream
+    EXL2B_CUDA(cudaMalloc(&p, (size_t)q->v.K * sizeof(half)));
+    gather_rows_kernel<<<(q->v.K + 255) / 256, 256>>>(p, norm_w, q->v.perm, q->v.K);
+    g_launch_count++;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) {
+        cudaFree(p);
+        EXL2B_CUDA(e);
     }
-    *out = q->normp_buf;
+    *out = p;
     return 0;
 }
 
@@ -963,11 +965,9 @@ int gemv_i8_launch(int device, cudaStream_t stream, const I8Out* outs, int nm, c
     P.norm_eps = in.norm_eps;
     P.mode = in.mode;
     P.x_permuted = in.x_permuted;
-    if (in.mode == I8_RMSNORM && P.perm) {
-        const half* wp = nullptr;
-        int rcn = i8_permuted_norm(const_cast<QMatrix*>(outs[0].q), in.norm_w, stream, &wp);
-        if (rcn) return rcn;
-        if (wp) { P.norm_w = wp; P.norm_permuted = 1; }
+    if (in.mode == I8_RMSNORM && P.perm && in.norm_wp) {
+        P.norm_w = in.norm_wp;
+        P.norm_permuted = 1;
     }
     I8PlanMat pm[I8_MAX_MATS];
     memset(pm, 0, sizeof(pm));

@@ -21,6 +21,8 @@ struct I8Input {
     float norm_eps;
     int mode;
     int x_permuted;       // x / x2 are already in the matrices' stored-row order (written by a producer launch's c_perm)
+    const half* norm_wp;  // norm_w in the matrices' stored-row order (permuted_norm_copy, owned by a block handle), or NULL:
+                          //   the kernel gathers norm_w through the permutation itself
 };
 
 struct I8Out {
@@ -35,6 +37,8 @@ struct I8Out {
 int gemv_i8_launch(int device, cudaStream_t stream, const I8Out* outs, int nm, const I8Input& in);
 // same K / same permutation contents / LAYOUT_TC?  (host check, synchronises once; call at block-creation time)
 bool gemv_i8_fusable(const QMatrix* const* qs, int nm);
+// a new device copy of norm_w[perm[k]] in q's stored-row order (cudaFree it); synchronises, never call inside a capture
+int permuted_norm_copy(const QMatrix* q, const half* norm_w, half** out);
 // EXL2B_GEMV=tc in the environment routes single rows through the wgmma kernel (gemm_tc.cu) instead (A/B comparisons)
 bool gemv_i8_enabled();
 

@@ -489,7 +489,6 @@ extern "C" int exl2b_qmatrix_destroy(exl2b_qmatrix_t h) {
     if (m->tables) cudaFree(m->tables);
     if (m->owned_packed) cudaFree(m->owned_packed);
     if (m->wtab) cudaFree(m->wtab);
-    if (m->normp_buf) cudaFree(m->normp_buf);
     if (m->xp_buf) cudaFree(m->xp_buf);
     if (m->sumsq_buf) cudaFree(m->sumsq_buf);
     delete m;

@@ -48,8 +48,6 @@ struct QMatrix {
     const uint16_t* invperm = nullptr;  // q_invperm of the checkpoint (device), NULL = identity
     void* wtab = nullptr;               // dense per-(group, column) scale table of the batch-1 GEMV (gemv_i8.cu): EXL2 fp16[G][N] =
                                         //   dq_scale(q_scale nibble, q_scale_max); GPTQ uint32[G][N] = fp16 scale | (qzero + 1) << 16
-    const half* normp_src = nullptr;    // batch-1 GEMV: the RMSNorm weight last used in front of this matrix, and that weight in the
-    half* normp_buf = nullptr;          //   matrix' stored-row order (norm_w[perm[k']]), built on first use
     half* xp_buf = nullptr;             // chained launches: this matrix's input, written by its producer's epilogue
     float* sumsq_buf = nullptr;         //   and the producer's per-strip sums of squares (deferred RMSNorm)
 };

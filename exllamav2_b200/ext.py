@@ -93,6 +93,7 @@ _sig("exl2b_qmlp_forward_gateup", c_int, c_void_p, c_void_p, c_int, c_void_p, c_
 _sig("exl2b_paged_attn_decode_q", c_int, *([c_void_p] * 10 + [c_int] * 7 + [c_float, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]))
 _sig("exl2b_paged_attn_status", c_int, c_int, POINTER(c_int))
 _sig("exl2b_paged_attn_clear_status", c_int, c_int)
+_sig("exl2b_debug_scratch", c_int, c_int, c_void_p, c_int, POINTER(c_void_p), POINTER(ctypes.c_size_t))
 
 
 class _Chain(Structure):
@@ -593,6 +594,20 @@ def paged_attn_status(device) -> int:
     st = c_int(0)
     _check(lib.exl2b_paged_attn_status(torch.device(device).index or 0, ctypes.byref(st)))
     return st.value
+
+
+# include/exl2_b200.h EXL2B_SCRATCH_*
+SCRATCH_KINDS = {"attn_ws": 0, "attn_cnt": 1, "tc_ws": 2, "tc_cnt": 3, "tc_xp": 4}
+
+
+def debug_scratch(device, stream, kind: str) -> tuple[int, int]:
+    """(device address, bytes) of the scratch a kernel family keeps for (device, stream) -- `kind` one of SCRATCH_KINDS --
+    or (0, 0) before the first launch that creates it.  `stream` is a torch.cuda.Stream or a raw cudaStream_t handle."""
+    handle = stream.cuda_stream if hasattr(stream, "cuda_stream") else int(stream)
+    ptr, nbytes = c_void_p(), ctypes.c_size_t()
+    _check(lib.exl2b_debug_scratch(torch.device(device).index or 0, handle or None, SCRATCH_KINDS[kind], ctypes.byref(ptr),
+                                   ctypes.byref(nbytes)))
+    return ptr.value or 0, nbytes.value
 
 
 HOT_PATH_EXPORTS = [

@@ -132,7 +132,8 @@ int exl2b_q_to_fp16_kv(const uint8_t* k_in, const uint16_t* k_scales, uint16_t* 
  * forward_1: RMSNorm(x) -> Q,K,V projections -> RoPE on Q and K; forward_2: x (+)= attn_out @ o_proj.
  * RMSNorm is folded into the projection kernel's prologue and Q/K/V run as ONE launch (SURVEY.md 7 step 3). */
 typedef struct exl2b_qattn_desc {
-    const uint16_t* layernorm;   /* fp16[hidden] RMSNorm weight or NULL */
+    const uint16_t* layernorm;   /* fp16[hidden] RMSNorm weight or NULL; the single-row path reads a copy taken at create
+                                    (here and in exl2b_qmlp_desc): recreate the handle after changing the weight */
     float norm_epsilon;
     exl2b_qmatrix_t q_proj, k_proj, v_proj, o_proj;
     int hidden_size, num_heads, num_kv_heads, head_dim;
@@ -189,6 +190,17 @@ int exl2b_debug_plan(int N, int KS, int is_gptq, uint32_t blk_stream_bytes, cons
  * group_base, off_base) per region.  info: CTAs, descriptors, arena bytes, scale-slot bytes, shared-memory bytes, longest list. */
 int exl2b_debug_i8_plan(const int* mats, int nm, int ctas, int warps, uint32_t* desc, int cap_desc, uint32_t* first, int cap_first,
                         int* info);
+/* diagnostics: the device scratch a kernel family keeps for (device, stream) -- its address and size, or NULL / 0 before
+ * the first launch that creates it.  Attention scratch is sized at its bound when created and never moves, so a graph
+ * captured on the stream keeps valid pointers; the wgmma activation scratch (TC_XP) grows with the row count. */
+enum {
+    EXL2B_SCRATCH_ATTN_WS = 0,   /* split-KV partial results of the fused decode attention */
+    EXL2B_SCRATCH_ATTN_CNT = 1,  /* its per-(sequence, head) arrival counters */
+    EXL2B_SCRATCH_TC_WS = 2,     /* split-K workspace of the wgmma kernel */
+    EXL2B_SCRATCH_TC_CNT = 3,    /* its arrival counters */
+    EXL2B_SCRATCH_TC_XP = 4,     /* its activation-operand scratch */
+};
+int exl2b_debug_scratch(int device, exl2b_stream_t stream, int kind, void** ptr, size_t* bytes);
 
 /* Stand-in for flash_attn_with_kvcache (third-party in the reference, attn.py:602-613): appends the q_len new K/V rows
  * to the paged fp16 cache at [seqlen, seqlen+q_len) and attends causally.  q [batch,q_len,H,hd], k/v_new

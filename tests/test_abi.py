@@ -51,6 +51,21 @@ def test_error_message_plumbing(lib):
     assert b"null handle" in lib.exl2b_last_error()
 
 
+def test_debug_scratch_query():
+    """exl2b_debug_scratch reports nothing for a (device, stream) no launch has used, names every kind the header declares,
+    and refuses an unknown kind; it never creates scratch, so it runs without a GPU."""
+    from exllamav2_b200 import ext as ext_c
+    hdr = open(os.path.join(ROOT, "include", "exl2_b200.h")).read()
+    declared = {m.group(1).lower(): int(m.group(2)) for m in re.finditer(r"EXL2B_SCRATCH_([A-Z_]+) = (\d+)", hdr)}
+    assert declared == ext_c.SCRATCH_KINDS
+    for kind in ext_c.SCRATCH_KINDS:
+        assert ext_c.debug_scratch("cuda:0", 0xDEAD000, kind) == (0, 0)
+    ptr, nbytes = ctypes.c_void_p(), ctypes.c_size_t()
+    assert ext_c.lib.exl2b_debug_scratch(0, None, len(declared), ctypes.byref(ptr), ctypes.byref(nbytes)) != 0
+    assert b"unknown scratch kind" in ext_c.lib.exl2b_last_error()
+    assert ext_c.lib.exl2b_debug_scratch(0, None, 0, None, ctypes.byref(nbytes)) != 0
+
+
 def test_hot_path_names_cover_reference_call_sites():
     """Every ext_c.<name> the reference's hot-path files call for a Llama-family quantized model must exist in our
     module (SURVEY.md 8b).  The names are stored in tests/golden/ref_ext_calls.json: every `ext_c.<name>(` call in the
