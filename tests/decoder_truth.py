@@ -10,6 +10,7 @@ drifted across a quantisation step.  The call's own tokens enter attention unqua
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
 
 import numpy as np
@@ -118,3 +119,320 @@ class TruthModel:
 
 def _round16(a: np.ndarray) -> np.ndarray:
     return np.asarray(a).astype(np.float16).astype(F64)
+
+
+# ---- the same forward in torch fp64, for models whose fp64 weights do not fit anywhere --------------------------------------
+# Weights stay in whatever dtype the caller holds them (the decoder's fp16 reconstruct() on the GPU); every product converts one
+# column chunk of at most CHUNK_BYTES of fp64 at a time, so a 70B-shaped layer never exists in fp64 as a whole.
+
+CHUNK_BYTES = 512 << 20
+
+
+def mm64(a, w, chunk_bytes: int = CHUNK_BYTES):
+    """a [T, K] @ w [K, N] in fp64, w converted to fp64 one column chunk at a time."""
+    import torch
+    a = a.to(torch.float64)
+    K, N = w.shape
+    cols = max(1, chunk_bytes // (8 * K))
+    out = torch.empty((a.shape[0], N), dtype=torch.float64, device=a.device)
+    for j0 in range(0, N, cols):
+        out[:, j0:j0 + cols] = a @ w[:, j0:j0 + cols].to(torch.float64)
+    return out
+
+
+class TorchTruthModel:
+    """TruthModel.forward restated in torch fp64 on `device` (tests/test_decoder_truth_model.py pins the two together).  layers:
+    TruthLayer-like objects whose matrices are torch tensors [K, N] of any float dtype; the result is a numpy CallTruth."""
+
+    def __init__(self, layers: list, final_norm, head, embed, sin, cos, num_heads: int, num_kv_heads: int, head_dim: int,
+                 eps: float, device, chunk_bytes: int = CHUNK_BYTES):
+        import torch
+        f = lambda t: torch.as_tensor(t).to(device=device, dtype=torch.float64)
+        self.layers = layers
+        self.norms = [(f(L.input_norm), f(L.post_norm)) for L in layers]
+        self.final_norm, self.head, self.embed = f(final_norm), head, torch.as_tensor(embed).to(device)     # rows converted when read
+        self.sin, self.cos = f(sin), f(cos)
+        self.H, self.KVH, self.hd, self.eps, self.device = num_heads, num_kv_heads, head_dim, eps, device
+        self.chunk = chunk_bytes
+
+    def _norm(self, x, w):
+        return x / (x * x).mean(-1, keepdim=True).add(self.eps).sqrt() * w
+
+    def _rope(self, x, pos):
+        import torch
+        h = x.shape[-1] // 2
+        c, s = self.cos[pos, :h][:, None, :], self.sin[pos, :h][:, None, :]
+        l, r = x[..., :h], x[..., h:]
+        return torch.cat([l * c - r * s, r * c + l * s], dim=-1)
+
+    def forward(self, ids, start: int, past_k: list, past_v: list, fp16: bool = False) -> CallTruth:
+        import torch
+        ids = np.asarray(ids).reshape(-1)
+        T = ids.shape[0]
+        H, KVH, hd = self.H, self.KVH, self.hd
+        r = (lambda a: a.half().double()) if fp16 else (lambda a: a)
+        pos = torch.as_tensor(start + np.arange(T), device=self.device)
+        x = self.embed[torch.as_tensor(ids, device=self.device)].to(torch.float64)
+        ks, vs = [], []
+        mask = torch.arange(start + T, device=self.device)[None, :] > pos[:, None]
+        for li, L in enumerate(self.layers):
+            n1, n2 = self.norms[li]
+            assert past_k[li].shape[0] == start and past_v[li].shape[0] == start
+            xn = r(self._norm(x, n1))
+            q = r(self._rope(r(mm64(xn, L.wq, self.chunk)).view(T, H, hd), pos))
+            k = r(self._rope(r(mm64(xn, L.wk, self.chunk)).view(T, KVH, hd), pos))
+            v = r(mm64(xn, L.wv, self.chunk).view(T, KVH, hd))
+            ks.append(k.cpu().numpy())
+            vs.append(v.cpu().numpy())
+            kc = torch.cat([torch.as_tensor(np.asarray(past_k[li], dtype=F64), device=self.device), k])
+            vc = torch.cat([torch.as_tensor(np.asarray(past_v[li], dtype=F64), device=self.device), v])
+            kk = kc.repeat_interleave(H // KVH, dim=1)          # head h reads kv head h // (H / KVH)
+            vv = vc.repeat_interleave(H // KVH, dim=1)
+            s = torch.einsum("thd,nhd->htn", q, kk) / math.sqrt(hd)
+            s = s.masked_fill(mask[None], -math.inf)
+            p = torch.softmax(s, dim=-1)
+            o = r(torch.einsum("htn,nhd->thd", p, vv).reshape(T, H * hd))
+            x = r(x + r(mm64(o, L.wo, self.chunk)))
+            xn = r(self._norm(x, n2))
+            g, u = r(mm64(xn, L.wg, self.chunk)), r(mm64(xn, L.wu, self.chunk))
+            a = r(g / (1.0 + torch.exp(-g)) * u)
+            x = r(x + r(mm64(a, L.wd, self.chunk)))
+        logits = mm64(self._norm(x, self.final_norm), self.head, self.chunk)
+        return CallTruth(hidden=x.cpu().numpy(), logits=logits.cpu().numpy(), k=ks, v=vs)
+
+
+# ---- which host branch a decoder call ran (shared by the GPU decoder tests) ------------------------------------------------------------------------------------------------
+
+SPIED = ["q_attn_forward_1", "q_attn_forward_1_ex", "paged_attn_decode_q4", "q_mlp_forward_", "q_mlp_forward_ex",
+         "q_mlp_forward_rows", "gemv_norm", "gemm_half_q_half_prepared", "gemm_half_q_half", "rms_norm", "q_to_fp16_kv",
+         "fp16_to_q_kv"]
+
+
+class Spy:
+    """Records the extension entry points the decoder calls (name, args, kwargs) without changing what they do."""
+
+    def __init__(self, monkeypatch):
+        from exllamav2_b200 import ext, model
+        self.calls = []
+        for name in SPIED:
+            monkeypatch.setattr(ext, name, self._wrap(name, getattr(ext, name)))
+        monkeypatch.setattr(model, "_sdpa_prefill", self._wrap("_sdpa_prefill", model._sdpa_prefill))
+        monkeypatch.setattr(model._lib, "exl2b_paged_attn_decode", self._wrap("exl2b_paged_attn_decode", model._lib.exl2b_paged_attn_decode))
+
+    def _wrap(self, name, fn):
+        def w(*a, **kw):
+            self.calls.append((name, a, kw))
+            return fn(*a, **kw)
+        return w
+
+    def take(self):
+        c, self.calls = self.calls, []
+        return c
+
+
+def named(calls, name):
+    return [(a, kw) for n, a, kw in calls if n == name]
+
+
+def names_of(calls):
+    return {n for n, _, _ in calls}
+
+
+def check_branch(sched, kind, calls, dec, L):
+    """Assert the host branch a call took, from the entry points it reached."""
+    from exllamav2_b200 import ext, model
+    B = dec.batch_size
+    # above one row the chained schedule runs every matrix on the wgmma kernel: a model with a matrix it cannot stage takes the
+    # fused, un-chained branch there instead (D5 as D3 / D6, P1 through q_attn_forward_1)
+    staged = all(ext.qmatrix_tc_supported(l.q_handle) for l in dec.linears)
+    if not staged and sched == "D5":
+        sched = "D6"
+    names = names_of(calls)
+    attn1 = named(calls, "q_attn_forward_1")
+    attn1_ex = named(calls, "q_attn_forward_1_ex")
+    fused = named(calls, "paged_attn_decode_q4")
+    ref_attn = named(calls, "exl2b_paged_attn_decode")
+    rows1 = sorted({a[2] * a[3] for a, _ in attn1})          # batch_size * q_len of q_attn_forward_1
+    if sched == "L" and kind == "decode":                    # the long case decodes in the benchmarked step
+        sched = "D1"
+    if kind == "decode":
+        head = {"gemv_norm", "gemm_half_q_half_prepared", "gemm_half_q_half"} & names
+        if sched == "D1":
+            assert dec.row_gemv and dec.chained and dec.fused_attn and B == 1
+            assert len(attn1_ex) == L and all(a[9] is None for a, _ in attn1_ex), "RoPE must be left to the attention kernel"
+            assert len(fused) == L and all(kw.get("rope") is not None for _, kw in fused)
+            assert head == {"gemv_norm"} and named(calls, "gemv_norm")[0][1].get("prepared") is True
+        elif sched in ("D2", "D5"):
+            assert dec.chained and dec.fused_attn and B <= 8 and (B > 1 or not dec.row_gemv)
+            assert len(attn1_ex) == L and all(a[9] is not None and a[2] == B for a, _ in attn1_ex)
+            assert len(fused) == L and all(kw.get("rope") is None for _, kw in fused)
+            assert head == {"gemm_half_q_half_prepared"}
+        elif sched in ("D3", "D6"):
+            assert dec.fused_attn and not (dec.chained and B <= 8 and staged)
+            assert not attn1_ex and rows1 == [B] and len(fused) == L and len(named(calls, "q_mlp_forward_")) == L
+            assert head == {"gemm_half_q_half"} and "rms_norm" in names
+            if sched == "D6" and staged:
+                assert 8 < B <= 16          # the 9..16-row wgmma, not the many-row path
+        elif sched == "D4":
+            assert not dec.fused_attn and not fused and len(ref_attn) == L
+            assert len(named(calls, "q_to_fp16_kv")) == L and len(named(calls, "fp16_to_q_kv")) == L
+            assert head == {"gemm_half_q_half"} and "rms_norm" in names
+        else:
+            raise KeyError(sched)
+        return
+    if kind == "prefill":
+        qlens = [a[3] for a, _ in attn1_ex] + [a[3] for a, _ in attn1]
+        if sched == "P1":
+            assert dec.chained and dec.fused_attn and B == 1
+            if staged:
+                assert not attn1 and [a[3] for a, _ in attn1_ex] == [8] * L + [3] * L
+            else:
+                assert not attn1_ex and [a[3] for a, _ in attn1] == [8] * L + [3] * L
+                assert [a[0].shape[1] for a, _ in fused] == [8] * L + [3] * L
+            assert "gemv_norm" not in names and "gemm_half_q_half_prepared" not in names
+        elif sched == "P2":
+            assert dec.fused_attn and B == 3
+            assert not attn1_ex and [a[2] * a[3] for a, _ in attn1] == [24] * L + [9] * L   # 24 > 16: gemm_big; 9: wgmma
+            assert [a[0].shape[1] for a, _ in fused] == [8] * L + [3] * L
+        elif sched == "P4":
+            assert not dec.fused_attn and not fused and ref_attn and max(qlens) <= 8
+            assert len(named(calls, "q_to_fp16_kv")) == len(ref_attn) == len(named(calls, "fp16_to_q_kv"))
+        # (prompts of decode schedules run in the decode schedule's flags; their numbers are checked all the same)
+        return
+    assert kind == "rows"
+    assert len(named(calls, "q_to_fp16_kv")) == L and len(named(calls, "fp16_to_q_kv")) == L
+    assert len(attn1) == L and len(named(calls, "q_mlp_forward_rows")) == L
+    assert len(named(calls, "_sdpa_prefill")) == (L if model._flash_attn_with_kvcache() is None else 0)
+
+
+# ---- checks of one decoder call, shared by the GPU decoder tests ---------------------------------------------------------------
+
+# rel-L2 of the decoder's output vs the fp64 truth, per schedule: about 2x the worst measured on an H100 (DESIGN.md §3.6)
+OUT_TOL = {"D1": 5e-3, "D2": 5e-3, "D3": 5e-3, "D4": 3e-3, "D5": 9e-3, "D6": 1e-2,
+           "P1": 5e-3, "P2": 7e-3, "P3": 6e-3, "P4": 4e-3, "L": 6e-3}
+# appended cache rows: |unpack(stored) - truth| <= KV_RATIO * |unpack(pack(fp16(truth))) - truth| + KV_SLACK * |truth|
+KV_RATIO = 1.1
+KV_SLACK = 2e-3
+# The fp16 floor of a call: how far the ideal fp16-storage forward (fp16=True) lies from the exact one on the same input.  It is
+# <= FLOOR_TYPICAL on almost every input; where the residual stream cancels it is several times larger, and so is any fp16
+# implementation's error there (on the hd-128 model some decode steps have a floor of 1-2e-2).  The output bound of a call scales
+# by floor / FLOOR_TYPICAL above that, and an appended cache row may be off by FLOOR_RATIO x its own floor.
+FLOOR_TYPICAL = 3e-3
+FLOOR_RATIO = 3.0
+
+
+def snapshot(dec):
+    c = dec.cache
+    return dict(k=[t.cpu().numpy().copy() for t in c.key_states], ks=[t.cpu().numpy().copy() for t in c.key_scales],
+                v=[t.cpu().numpy().copy() for t in c.value_states], vs=[t.cpu().numpy().copy() for t in c.value_scales],
+                seqlens=c.cache_seqlens.cpu().numpy().copy(), bt=c.block_table.cpu().numpy().copy())
+
+
+def slots(snap, b, lo, hi):
+    from exllamav2_b200.model import PAGE_SIZE
+    p = np.arange(lo, hi)
+    return snap["bt"][b][p // PAGE_SIZE], p % PAGE_SIZE
+
+
+def cache_kv(snap, cfg, bits, li, b, lo, hi):
+    """Dequantised K and V of sequence b, positions [lo, hi), layer li: [n, KVH, hd] fp64, following the stored page table."""
+    import kv_q68
+    n, shp = hi - lo, (hi - lo, cfg.num_kv_heads, cfg.head_dim)
+    if n == 0:
+        return np.zeros(shp), np.zeros(shp)
+    pg, r = slots(snap, b, lo, hi)
+    kb, vb = kv_q68.widths(bits)
+    k = kv_q68.kv_unpack(snap["k"][li][pg, r].reshape(n, -1), snap["ks"][li][pg, r].reshape(n, -1), kb)
+    v = kv_q68.kv_unpack(snap["v"][li][pg, r].reshape(n, -1), snap["vs"][li][pg, r].reshape(n, -1), vb)
+    return k.astype(np.float64).reshape(shp), v.astype(np.float64).reshape(shp)
+
+
+def row_err(stored, truth, b):
+    """(|stored - truth|, |unpack(pack(fp16(truth))) - truth|, |truth|) per row; rows [n, KVH, hd]."""
+    import kv_q68
+    t = truth.reshape(truth.shape[0], -1)
+    rq = kv_q68.kv_unpack(*kv_q68.kv_pack(t.astype(np.float16), b), b).astype(np.float64)
+    s = stored.reshape(t.shape)
+    return np.linalg.norm(s - t, axis=1), np.linalg.norm(rq - t, axis=1), np.linalg.norm(t, axis=1)
+
+
+def check_call(dec, truth, sched, kind, ids, out, pre, post, pos0, chunk=8, floor_ratio=0.0):
+    """What every checked decoder call must satisfy, given the cache snapshots before (pre) and after (post) it and its output
+    (decode: logits [B, vocab]; prompt: hidden state [B, T_last, hidden]):
+      (3) cache_seqlens and dec.pos advanced by exactly the tokens fed, the page table untouched;
+      (2a) cache bytes at positions written before the call unchanged;
+      (2b) each appended row, dequantised, within KV_RATIO x the format's own quantisation error of the truth row (+ slack,
+           or FLOOR_RATIO x that row's fp16 floor);
+      (1) the output per sequence within OUT_TOL[sched] rel-L2 of the truth, scaled up by floor / FLOOR_TYPICAL where this
+          input's fp16 floor is larger than that, and never below floor_ratio x the floor (0: off).
+    Returns (worst output rel-L2, worst floor, number of sequences whose bound was scaled)."""
+    import kv_q68
+    from exl2_oracle import rel_l2
+    cfg, bits = dec.cfg, dec.cache.wbits
+    B, T = ids.shape
+    L = cfg.num_layers
+    assert np.array_equal(post["seqlens"], pre["seqlens"] + T), (pre["seqlens"], post["seqlens"], T)
+    assert dec.pos == pos0 + T
+    assert np.array_equal(post["bt"], pre["bt"])
+    assert np.isfinite(out).all()
+    kb, vb = kv_q68.widths(bits)
+    worst, worst_floor, floored = 0.0, 0.0, 0
+    chunks = [(t0, min(chunk, T - t0)) for t0 in range(0, T, chunk)] if kind == "prefill" else [(0, T)]
+    for b in range(B):
+        pg, r = slots(pre, b, 0, pos0)
+        for key in ("k", "ks", "v", "vs"):
+            for li in range(L):
+                assert np.array_equal(post[key][li][pg, r], pre[key][li][pg, r]), f"seq {b} layer {li}: {key} of the past changed"
+        for t0, n in chunks:
+            start = pos0 + t0
+            past = [cache_kv(post, cfg, bits, li, b, 0, start) for li in range(L)]
+            pk, pv = [p[0] for p in past], [p[1] for p in past]
+            res = truth.forward(ids[b, t0:t0 + n], start, pk, pv)
+            res16 = truth.forward(ids[b, t0:t0 + n], start, pk, pv, fp16=True)
+            for li in range(L):
+                k, v = cache_kv(post, cfg, bits, li, b, start, start + n)
+                for got, want, want16, wb, what in ((k, res.k[li], res16.k[li], kb, "K"), (v, res.v[li], res16.v[li], vb, "V")):
+                    e, eq, nt = row_err(got, want, wb)
+                    floor = np.linalg.norm((want16 - want).reshape(n, -1), axis=1)
+                    bad = e > KV_RATIO * eq + np.maximum(KV_SLACK * nt, FLOOR_RATIO * floor)
+                    assert not bad.any(), (f"seq {b} layer {li} {what} rows {start + np.flatnonzero(bad)}: error "
+                                           f"{e[bad] / nt[bad]} vs quantisation {eq[bad] / nt[bad]}, fp16 floor {floor[bad] / nt[bad]}")
+        want, want16 = (res.logits[-1], res16.logits[-1]) if kind == "decode" else (res.hidden, res16.hidden)
+        err, floor = rel_l2(out[b], want), rel_l2(want16, want)
+        bound = max(OUT_TOL[sched] * max(1.0, floor / FLOOR_TYPICAL), floor_ratio * floor)
+        floored += bound > OUT_TOL[sched]
+        worst, worst_floor = max(worst, err), max(worst_floor, floor)
+        assert err <= bound, f"{sched} seq {b}: rel-L2 {err:.3e} vs the fp64 truth (bound {bound:.3e}, fp16 floor {floor:.3e})"
+    return worst, worst_floor, floored
+
+
+def graph_matches_eager(dec, ids, on_eager=None):
+    """One decode step eagerly, then the same step (same cache state) by graph replay: identical logits and cache bytes.  Leaves
+    the decoder as it was, with the graph armed.  on_eager() runs right after the eager step (the caller's branch check)."""
+    import torch
+    c = dec.cache
+    live = (*c.key_states, *c.key_scales, *c.value_states, *c.value_scales, c.cache_seqlens)
+    state = [t.clone() for t in live]
+
+    def restore():
+        for dst, src in zip(live, state):
+            dst.copy_(src)
+
+    g, dec.graph = dec.graph, None
+    x = torch.from_numpy(ids).to(c.cache_seqlens.device)
+    eager = dec.decode(x).clone()
+    eager_cache = snapshot(dec)
+    if on_eager is not None:
+        on_eager()
+    restore()
+    dec.pos -= 1
+    dec.graph = g
+    replay = dec.decode(x).clone()
+    replay_cache = snapshot(dec)
+    assert torch.equal(eager.view(torch.int16), replay.view(torch.int16)), "graph replay differs from the eager step"
+    for key in ("k", "ks", "v", "vs"):
+        for a, b in zip(eager_cache[key], replay_cache[key]):
+            assert np.array_equal(a.view(np.uint8), b.view(np.uint8)), f"graph replay stored different {key}"
+    assert np.array_equal(eager_cache["seqlens"], replay_cache["seqlens"])
+    restore()
+    dec.pos -= 1

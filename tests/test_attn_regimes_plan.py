@@ -33,6 +33,23 @@ def test_nsplit():
     assert [(c["p_lo"], c["p_hi"]) for c in p["ctas"] if c["b"] == 2] == [(0, 501), (501, 1002), (1002, 1501)]
 
 
+@pytest.mark.parametrize("wbits", [4, 6, 8])
+def test_wide_head_layouts(wbits):
+    """The 70B preset's 64 heads and a 28-head GQA-7 model (the regimes test_gpu_attn_regimes adds for them): 2 * 132 // 64 = 4
+    chunks at B = 1, with the ring above 8192 positions; at B = 8 the 512 (head, sequence) CTAs outnumber the SMs and nothing
+    splits; 264 // 28 = 9 chunks of 512 positions over a 4608-position cache."""
+    p = ar.plan(wbits, 128, 64, 1, 1, 4096, [4095])
+    assert p["nsplit"] == 4 and not p["ring"] and ar.branches(p, 1, 64, 1) >= {"merge", "global"}
+    assert [(c["p_lo"], c["p_hi"]) for c in p["ctas"]] == [(z * 1024, z * 1024 + 1024) for z in range(4)]
+    p = ar.plan(wbits, 128, 64, 1, 1, 16384, [16383])
+    assert p["nsplit"] == 4 and p["ring"] and ar.branches(p, 1, 64, 1) >= {"merge", "ring"}
+    p = ar.plan(wbits, 128, 64, 8, 1, 4096, [0, 1, 255, 256, 513, 1500, 3000, 4095])
+    assert p["nsplit"] == 1 and ar.branches(p, 1, 64, 8) >= {"batched", "global"}
+    p = ar.plan(wbits, 128, 28, 1, 1, 4608, [4607])
+    assert p["nsplit"] == 9 and [(c["p_lo"], c["p_hi"]) for c in p["ctas"]] == [(z * 512, z * 512 + 512) for z in range(9)]
+    assert 28 * 9 <= 2 * ar.H100_SMS and 64 * 4 <= 2 * ar.H100_SMS        # within the split-KV scratch bound (attn_q4.cu)
+
+
 def _largest_fit(wbits, hd, q_len, B, H=32):
     pages = 1
     while ar.smem_bytes(wbits, hd, q_len, (pages + 1) * ar.PAGE, ar.nsplit_of(q_len, (pages + 1) * ar.PAGE, H, B))["fits"]:

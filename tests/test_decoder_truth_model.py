@@ -98,6 +98,31 @@ def test_forward_is_invariant_under_a_position_shift(H, KVH):
     assert np.abs(a.hidden - b.hidden).max() <= 1e-12 * np.abs(a.hidden).max()
 
 
+@pytest.mark.parametrize("H,KVH,hidden", [(4, 2, 64), (7, 1, 48), (14, 2, 160)], ids=["gqa2", "gqa7-narrow", "gqa7-wide"])
+@pytest.mark.parametrize("fp16", [False, True], ids=["exact", "fp16"])
+def test_torch_forward_equals_numpy_forward(H, KVH, hidden, fp16):
+    """The torch fp64 restatement the full-size GPU tests use (decoder_truth.TorchTruthModel, chunked products) is the numpy
+    forward, on CPU: GQA ratios of 2 and 7, attention wider (112 vs 48) and narrower (224 vs 160) than the hidden size, a past
+    of 6 positions, and column chunks small enough that every product takes several.  In fp16-storage mode a last-bit difference
+    of the two fp64 sums may round an intermediate to the neighbouring fp16 value, and one such flip moves these toy models by up
+    to ~4e-4, so there the two are held to 1e-3 rel-L2 instead of 1e-12."""
+    import torch
+    m = _model(H, KVH, hidden=hidden, seed=H * 100 + hidden)
+    tl = [dt.TruthLayer(**{f: torch.from_numpy(getattr(L, f)) for f in L.__dataclass_fields__}) for L in m.layers]
+    tm = dt.TorchTruthModel(tl, m.final_norm, torch.from_numpy(m.head), m.embed, m.sin, m.cos, m.H, m.KVH, m.hd, m.eps, "cpu",
+                            chunk_bytes=8 * 64 * 16)
+    ids = np.random.default_rng(6).integers(0, 50, size=10)
+    past = m.forward(ids[:6], 0, _empty(m), _empty(m))
+    a = m.forward(ids[6:], 6, past.k, past.v, fp16=fp16)
+    b = tm.forward(ids[6:], 6, past.k, past.v, fp16=fp16)
+    for x, y in ((a.logits, b.logits), (a.hidden, b.hidden), *zip(a.k, b.k), *zip(a.v, b.v)):
+        assert x.shape == y.shape
+        if fp16:
+            assert np.linalg.norm(x - y) <= 1e-3 * np.linalg.norm(x)
+        else:
+            assert np.abs(x - y).max() <= 1e-12 * max(1.0, np.abs(x).max())
+
+
 @pytest.mark.parametrize("H,KVH", [(4, 4), (4, 2)], ids=["mha", "gqa"])
 def test_fp16_storage_mode_is_a_rounding_level_perturbation(H, KVH):
     m = _model(H, KVH, seed=11)

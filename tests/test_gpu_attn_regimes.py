@@ -75,10 +75,22 @@ def regime(name, wbits, hd):
     if name == "batched":
         sl = [0, 1, 255, 256, 511, 512, 513, 4095] + ([3000] if hd == 128 else [])
         return dict(H=32, KVH=8, q_len=1, max_ctx=4096, seqlens=sl, expect={"batched", "global"})
+    # the 70B preset's heads (H 64, KVH 8): 264 / 64 = 4 chunks at B = 1, and at B = 8 more CTAs than SMs without split
+    if name == "heads64_q1":
+        return dict(H=64, KVH=8, q_len=1, max_ctx=4096, seqlens=[4095], expect={"merge", "global"}, nsplit=4)
+    if name == "heads64_ring":
+        return dict(H=64, KVH=8, q_len=1, max_ctx=16384, seqlens=[16383], expect={"merge", "ring"}, nsplit=4)
+    if name == "heads64_batched":
+        return dict(H=64, KVH=8, q_len=1, max_ctx=4096, seqlens=[0, 1, 255, 256, 513, 1500, 3000, 4095],
+                    expect={"batched", "global"}, nsplit=1)
+    # a GQA ratio that is not a power of two (Qwen2.5-7B: 28 heads over 4 kv heads): 264 / 28 = 9 chunks of 512 positions
+    if name == "gqa7_split9":
+        return dict(H=28, KVH=4, q_len=1, max_ctx=4608, seqlens=[4607], expect={"merge"}, nsplit=9)
     raise KeyError(name)
 
 
 REGIMES = ["global_qlen", "global_q1", "ring", "ring_qlen", "split_batch", "split_batch3", "batched"]
+WIDE = ["heads64_q1", "heads64_ring", "heads64_batched", "gqa7_split9"]      # hd 128 only, the head dim of the models they stand for
 
 
 def ek_of(h, group, hd):
@@ -109,6 +121,7 @@ def base_case(wbits, hd, name, sigma_key=None, beta=BETA):
     p = ar.plan(wbits, hd, H, B, q_len, max_ctx, seqlens)
     got = ar.branches(p, q_len, H, B)
     assert r["expect"] <= got, (name, r["expect"], got)
+    assert p["nsplit"] == r.get("nsplit", p["nsplit"]), (name, p["nsplit"])
     sigma = sigma_key if sigma_key is not None else 1.0 / np.sqrt(hd)
     rng = np.random.default_rng(stable_seed(wbits, hd, name))
     pages_total = B * pps + 1                      # one page no sequence owns: nothing may write it
@@ -264,7 +277,8 @@ def needle_mask(c, b, h, extra=()):
     return m
 
 
-CASES = [(w, hd, name, mode) for (w, hd) in FMTS for name in REGIMES for mode in ("random", "needle", "zero")]
+CASES = [(w, hd, name, mode) for (w, hd) in FMTS for name in REGIMES + WIDE for mode in ("random", "needle", "zero")
+         if hd == 128 or name not in WIDE]
 
 
 @pytest.mark.parametrize("wbits,hd,name,mode", CASES)
@@ -303,14 +317,17 @@ def _chunks(c, b):
     return [(x["p_lo"], x["p_hi"]) for x in c["plan"]["ctas"] if x["b"] == b]
 
 
-@pytest.mark.parametrize("wbits,hd", FMTS)
+SKEW_CASES = [(w, hd, "split_batch") for (w, hd) in FMTS] + [(w, 128, n) for w in (4, 6, 8) for n in ("heads64_q1", "gqa7_split9")]
+
+
+@pytest.mark.parametrize("wbits,hd,name", SKEW_CASES)
 @pytest.mark.parametrize("skew", ["sink", "deep", "sink_last"])
-def test_skewed_merge(wbits, hd, skew):
+def test_skewed_merge(wbits, hd, name, skew):
     """Split-KV whose chunks' maxima differ widely.  sink: a needle 6 nats above the rest in the first chunk of every split
     sequence, the other chunks still carrying 1-10 % of the mass, so a merge that drops their rescale or weight fails.
     deep: the second chunk's rows all score ~100 nats below the rest; its merge weight underflows to zero and the output
-    stays finite.  sink_last: the sink is the appended row, in the last chunk."""
-    name = "split_batch"
+    stays finite.  sink_last: the sink is the appended row, in the last chunk.  Added needles skip positions that already hold
+    one (the plan's boundary needles), which with 64 heads fall inside the range they are spread over."""
     c0 = base_case(wbits, hd, name)
     c = dict(c0)
     kq, ks, vq, vs = (c0[k].copy() for k in ("kq", "ks", "vq", "vs"))
@@ -318,6 +335,14 @@ def test_skewed_merge(wbits, hd, skew):
     split = [b for b in range(c["B"]) if len(_chunks(c, b)) >= 3]
     assert split
     extra = []
+    taken = {(n[0], n[1]) for n in c0["needles"]}
+
+    def free(b, pos):
+        while (b, pos) in taken:
+            pos += 1
+        taken.add((b, pos))
+        return pos
+
     if skew in ("sink", "sink_last"):
         # three more needles of every head at S0 in each chunk the sink is not in: together they carry a few % of the mass
         for b in split:
@@ -325,7 +350,7 @@ def test_skewed_merge(wbits, hd, skew):
             for lo, hi in (ch[1:] if skew == "sink" else ch[:-1]):
                 for h in range(H):
                     for k in range(3):
-                        pos = lo + 20 + 4 * h + k
+                        pos = free(b, lo + 20 + 4 * h + k)
                         pg, rr, g = c["bt"][b, pos // ar.PAGE], pos % ar.PAGE, h // group
                         kq[pg, rr, g] = ar.s_one_hot_row(hd, kb, ek_of(h, group, hd))
                         ks[pg, rr, g, ek_of(h, group, hd) // 32] = key_scale(S0, sigma, c["beta"], kb)
@@ -334,7 +359,7 @@ def test_skewed_merge(wbits, hd, skew):
         for b in split:
             lo, hi = _chunks(c, b)[0]
             for h in range(H):
-                pos = lo + 100 + 3 * h                              # inside the first chunk, no boundary
+                pos = free(b, lo + 100 + 3 * h)                     # inside the first chunk, no boundary
                 pg, rr, g = c["bt"][b, pos // ar.PAGE], pos % ar.PAGE, h // group
                 kq[pg, rr, g] = ar.s_one_hot_row(hd, kb, ek_of(h, group, hd))
                 ks[pg, rr, g, ek_of(h, group, hd) // 32] = key_scale(S0 + 6.0, sigma, c["beta"], kb)
@@ -398,14 +423,16 @@ EDGES = {"pow2": 4.0, "guard_bumped": 2.0 * (2 - 2.0 ** -14), "below_guard": 2.0
          "just_below": 2.0 * (2 - 2.0 ** -23)}
 
 
-@pytest.mark.parametrize("wbits,hd", FMTS)
+EDGE_CASES = [(w, hd, "global_q1") for (w, hd) in FMTS] + [(w, 128, n) for w in (4, 6, 8) for n in ("heads64_q1", "gqa7_split9")]
+
+
+@pytest.mark.parametrize("wbits,hd,name", EDGE_CASES)
 @pytest.mark.parametrize("edge", list(EDGES))
-def test_query_block_max_at_power_of_two(wbits, hd, edge):
+def test_query_block_max_at_power_of_two(wbits, hd, name, edge):
     """rotate_q quantises each rotated 32-value query block to 16 bits under a power-of-two scale chosen from
     amax * 1.000030518, so the largest value stays inside the signed high byte.  The needle query's block maximum is put
     exactly on a power of two, just below it, and on both sides of that guard; the host's fp32 rotation confirms where it
     lands, and the needles' weights must still be read back within the usual tolerance."""
-    name = "global_q1"
     kb, _ = ar.widths(wbits)
     sigma, shave = _edge_query(EDGES[edge], hd, kb)
     c = base_case(wbits, hd, name, sigma_key=sigma, beta=1.0)

@@ -23,7 +23,7 @@ ungrouped act-order GPTQ plan (groups it cannot stage: above one row its steps t
 Q4 / Q6 / Q8.
 
 Per call: (1) logits (decode) or the returned hidden state (prompt) per sequence vs the fp64 truth, rel-L2 below a measured
-bound per schedule (DESIGN.md §3.6), scaled up only on inputs whose fp16 floor is atypically large (see FLOOR_TYPICAL);
+bound per schedule (DESIGN.md §3.6), scaled up only on inputs whose fp16 floor is atypically large (decoder_truth.FLOOR_TYPICAL);
 (2) cache bytes at positions written before the call unchanged, and each appended row, dequantised, no further from the truth
 row than 1.1x the format's own quantisation error of that row plus a small slack; (3) cache_seqlens and dec.pos advanced by
 exactly the tokens fed; (4) D1: graph replay produces eager's bits.  Each call also asserts the host branch it took, from the
@@ -36,25 +36,13 @@ import torch
 
 import decoder_truth as dt
 import exl2_oracle as oracle
-import kv_q68
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 SEED = 3
 CACHE_LEN = 512         # 2 pages per sequence
 
-# rel-L2 of the decoder's output vs the fp64 truth, per schedule: about 2x the worst measured on an H100 (DESIGN.md §3.6)
-OUT_TOL = {"D1": 5e-3, "D2": 5e-3, "D3": 5e-3, "D4": 3e-3, "D5": 9e-3, "D6": 1e-2,
-           "P1": 5e-3, "P2": 7e-3, "P3": 6e-3, "P4": 4e-3, "L": 6e-3}
-# appended cache rows: |unpack(stored) - truth| <= KV_RATIO * |unpack(pack(fp16(truth))) - truth| + KV_SLACK * |truth|
-KV_RATIO = 1.1
-KV_SLACK = 2e-3
-# The fp16 floor of a call: how far the ideal fp16-storage forward (decoder_truth fp16=True) lies from the exact one on the same
-# input.  It is <= FLOOR_TYPICAL on almost every input; where the residual stream cancels it is several times larger, and so is
-# any fp16 implementation's error there (on the hd-128 model some decode steps have a floor of 1-2e-2).  The output bound of a
-# call scales by floor / FLOOR_TYPICAL above that, and an appended cache row may be off by FLOOR_RATIO x its own floor.
-FLOOR_TYPICAL = 3e-3
-FLOOR_RATIO = 3.0
+OUT_TOL = dt.OUT_TOL     # per-schedule output bounds and the fp16-floor / K/V-row rules: tests/decoder_truth.py
 
 
 # ---- models -------------------------------------------------------------------------------------------------------------
@@ -176,145 +164,6 @@ def _in_child(request, row_gemv):
     return True
 
 
-# ---- cache access -------------------------------------------------------------------------------------------------------
-
-def _snapshot(dec):
-    c = dec.cache
-    return dict(k=[t.cpu().numpy().copy() for t in c.key_states], ks=[t.cpu().numpy().copy() for t in c.key_scales],
-                v=[t.cpu().numpy().copy() for t in c.value_states], vs=[t.cpu().numpy().copy() for t in c.value_scales],
-                seqlens=c.cache_seqlens.cpu().numpy().copy(), bt=c.block_table.cpu().numpy().copy())
-
-
-def _slots(snap, b, lo, hi):
-    from exllamav2_b200.model import PAGE_SIZE
-    p = np.arange(lo, hi)
-    return snap["bt"][b][p // PAGE_SIZE], p % PAGE_SIZE
-
-
-def _cache_kv(snap, cfg, bits, li, b, lo, hi):
-    """Dequantised K and V of sequence b, positions [lo, hi), layer li: [n, KVH, hd] fp64, following the stored page table."""
-    n, shp = hi - lo, (hi - lo, cfg.num_kv_heads, cfg.head_dim)
-    if n == 0:
-        return np.zeros(shp), np.zeros(shp)
-    pg, r = _slots(snap, b, lo, hi)
-    kb, vb = kv_q68.widths(bits)
-    k = kv_q68.kv_unpack(snap["k"][li][pg, r].reshape(n, -1), snap["ks"][li][pg, r].reshape(n, -1), kb)
-    v = kv_q68.kv_unpack(snap["v"][li][pg, r].reshape(n, -1), snap["vs"][li][pg, r].reshape(n, -1), vb)
-    return k.astype(np.float64).reshape(shp), v.astype(np.float64).reshape(shp)
-
-
-def _row_err(stored, truth, b):
-    """(|stored - truth|, |unpack(pack(fp16(truth))) - truth|, |truth|) per row; rows [n, KVH, hd]."""
-    t = truth.reshape(truth.shape[0], -1)
-    rq = kv_q68.kv_unpack(*kv_q68.kv_pack(t.astype(np.float16), b), b).astype(np.float64)
-    s = stored.reshape(t.shape)
-    return np.linalg.norm(s - t, axis=1), np.linalg.norm(rq - t, axis=1), np.linalg.norm(t, axis=1)
-
-
-# ---- which host branch ran ------------------------------------------------------------------------------------------------
-
-SPIED = ["q_attn_forward_1", "q_attn_forward_1_ex", "paged_attn_decode_q4", "q_mlp_forward_", "q_mlp_forward_ex",
-         "q_mlp_forward_rows", "gemv_norm", "gemm_half_q_half_prepared", "gemm_half_q_half", "rms_norm", "q_to_fp16_kv",
-         "fp16_to_q_kv"]
-
-
-class Spy:
-    """Records the extension entry points the decoder calls (name, args, kwargs) without changing what they do."""
-
-    def __init__(self, monkeypatch):
-        from exllamav2_b200 import ext, model
-        self.calls = []
-        for name in SPIED:
-            monkeypatch.setattr(ext, name, self._wrap(name, getattr(ext, name)))
-        monkeypatch.setattr(model, "_sdpa_prefill", self._wrap("_sdpa_prefill", model._sdpa_prefill))
-        monkeypatch.setattr(model._lib, "exl2b_paged_attn_decode", self._wrap("exl2b_paged_attn_decode", model._lib.exl2b_paged_attn_decode))
-
-    def _wrap(self, name, fn):
-        def w(*a, **kw):
-            self.calls.append((name, a, kw))
-            return fn(*a, **kw)
-        return w
-
-    def take(self):
-        c, self.calls = self.calls, []
-        return c
-
-
-def _named(calls, name):
-    return [(a, kw) for n, a, kw in calls if n == name]
-
-
-def _names(calls):
-    return {n for n, _, _ in calls}
-
-
-def _check_branch(sched, kind, calls, dec, L):
-    """Assert the host branch a call took, from the entry points it reached."""
-    from exllamav2_b200 import ext, model
-    B = dec.batch_size
-    # above one row the chained schedule runs every matrix on the wgmma kernel: a model with a matrix it cannot stage takes the
-    # fused, un-chained branch there instead (D5 as D3 / D6, P1 through q_attn_forward_1)
-    staged = all(ext.qmatrix_tc_supported(l.q_handle) for l in dec.linears)
-    if not staged and sched == "D5":
-        sched = "D6"
-    names = _names(calls)
-    attn1 = _named(calls, "q_attn_forward_1")
-    attn1_ex = _named(calls, "q_attn_forward_1_ex")
-    fused = _named(calls, "paged_attn_decode_q4")
-    ref_attn = _named(calls, "exl2b_paged_attn_decode")
-    rows1 = sorted({a[2] * a[3] for a, _ in attn1})          # batch_size * q_len of q_attn_forward_1
-    if sched == "L" and kind == "decode":                    # the long case decodes in the benchmarked step
-        sched = "D1"
-    if kind == "decode":
-        head = {"gemv_norm", "gemm_half_q_half_prepared", "gemm_half_q_half"} & names
-        if sched == "D1":
-            assert dec.row_gemv and dec.chained and dec.fused_attn and B == 1
-            assert len(attn1_ex) == L and all(a[9] is None for a, _ in attn1_ex), "RoPE must be left to the attention kernel"
-            assert len(fused) == L and all(kw.get("rope") is not None for _, kw in fused)
-            assert head == {"gemv_norm"} and _named(calls, "gemv_norm")[0][1].get("prepared") is True
-        elif sched in ("D2", "D5"):
-            assert dec.chained and dec.fused_attn and B <= 8 and (B > 1 or not dec.row_gemv)
-            assert len(attn1_ex) == L and all(a[9] is not None and a[2] == B for a, _ in attn1_ex)
-            assert len(fused) == L and all(kw.get("rope") is None for _, kw in fused)
-            assert head == {"gemm_half_q_half_prepared"}
-        elif sched in ("D3", "D6"):
-            assert dec.fused_attn and not (dec.chained and B <= 8 and staged)
-            assert not attn1_ex and rows1 == [B] and len(fused) == L and len(_named(calls, "q_mlp_forward_")) == L
-            assert head == {"gemm_half_q_half"} and "rms_norm" in names
-            if sched == "D6" and staged:
-                assert 8 < B <= 16          # the 9..16-row wgmma, not the many-row path
-        elif sched == "D4":
-            assert not dec.fused_attn and not fused and len(ref_attn) == L
-            assert len(_named(calls, "q_to_fp16_kv")) == L and len(_named(calls, "fp16_to_q_kv")) == L
-            assert head == {"gemm_half_q_half"} and "rms_norm" in names
-        else:
-            raise KeyError(sched)
-        return
-    if kind == "prefill":
-        qlens = [a[3] for a, _ in attn1_ex] + [a[3] for a, _ in attn1]
-        if sched == "P1":
-            assert dec.chained and dec.fused_attn and B == 1
-            if staged:
-                assert not attn1 and [a[3] for a, _ in attn1_ex] == [8] * L + [3] * L
-            else:
-                assert not attn1_ex and [a[3] for a, _ in attn1] == [8] * L + [3] * L
-                assert [a[0].shape[1] for a, _ in fused] == [8] * L + [3] * L
-            assert "gemv_norm" not in names and "gemm_half_q_half_prepared" not in names
-        elif sched == "P2":
-            assert dec.fused_attn and B == 3
-            assert not attn1_ex and [a[2] * a[3] for a, _ in attn1] == [24] * L + [9] * L   # 24 > 16: gemm_big; 9: wgmma
-            assert [a[0].shape[1] for a, _ in fused] == [8] * L + [3] * L
-        elif sched == "P4":
-            assert not dec.fused_attn and not fused and ref_attn and max(qlens) <= 8
-            assert len(_named(calls, "q_to_fp16_kv")) == len(ref_attn) == len(_named(calls, "fp16_to_q_kv"))
-        # (prompts of decode schedules run in the decode schedule's flags; their numbers are checked all the same)
-        return
-    assert kind == "rows"
-    assert len(_named(calls, "q_to_fp16_kv")) == L and len(_named(calls, "fp16_to_q_kv")) == L
-    assert len(attn1) == L and len(_named(calls, "q_mlp_forward_rows")) == L
-    assert len(_named(calls, "_sdpa_prefill")) == (L if model._flash_attn_with_kvcache() is None else 0)
-
-
 # ---- one call, checked ----------------------------------------------------------------------------------------------------
 
 def _call(dec, truth, sched, kind, ids, spy, chunk=8):
@@ -322,7 +171,7 @@ def _call(dec, truth, sched, kind, ids, spy, chunk=8):
     cfg, bits = dec.cfg, dec.cache.wbits
     B, T = ids.shape
     L = cfg.num_layers
-    pre = _snapshot(dec)
+    pre = dt.snapshot(dec)
     pos0 = dec.pos
     assert (pre["seqlens"] == pos0).all()
     spy.take()
@@ -336,45 +185,8 @@ def _call(dec, truth, sched, kind, ids, spy, chunk=8):
     torch.cuda.synchronize()
     calls = spy.take()
     if dec.graph is None:           # (a replayed step reaches no entry point: its eager twin is checked instead)
-        _check_branch(sched, kind, calls, dec, L)
-    post = _snapshot(dec)
-    # (3) bookkeeping
-    assert np.array_equal(post["seqlens"], pre["seqlens"] + T), (pre["seqlens"], post["seqlens"], T)
-    assert dec.pos == pos0 + T
-    assert np.array_equal(post["bt"], pre["bt"])
-    assert np.isfinite(out).all()
-    kb, vb = kv_q68.widths(bits)
-    worst, worst_floor, floored = 0.0, 0.0, 0
-    chunks = [(t0, min(chunk, T - t0)) for t0 in range(0, T, chunk)] if kind == "prefill" else [(0, T)]
-    for b in range(B):
-        # (2a) positions written before this call keep their bytes
-        pg, r = _slots(pre, b, 0, pos0)
-        for key in ("k", "ks", "v", "vs"):
-            for li in range(L):
-                assert np.array_equal(post[key][li][pg, r], pre[key][li][pg, r]), f"seq {b} layer {li}: {key} of the past changed"
-        for t0, n in chunks:
-            start = pos0 + t0
-            past = [_cache_kv(post, cfg, bits, li, b, 0, start) for li in range(L)]
-            pk, pv = [p[0] for p in past], [p[1] for p in past]
-            res = truth.forward(ids[b, t0:t0 + n], start, pk, pv)
-            res16 = truth.forward(ids[b, t0:t0 + n], start, pk, pv, fp16=True)
-            # (2b) the rows this chunk appended
-            for li in range(L):
-                k, v = _cache_kv(post, cfg, bits, li, b, start, start + n)
-                for got, want, want16, wb, what in ((k, res.k[li], res16.k[li], kb, "K"), (v, res.v[li], res16.v[li], vb, "V")):
-                    e, eq, nt = _row_err(got, want, wb)
-                    floor = np.linalg.norm((want16 - want).reshape(n, -1), axis=1)
-                    bad = e > KV_RATIO * eq + np.maximum(KV_SLACK * nt, FLOOR_RATIO * floor)
-                    assert not bad.any(), (f"seq {b} layer {li} {what} rows {start + np.flatnonzero(bad)}: error "
-                                           f"{e[bad] / nt[bad]} vs quantisation {eq[bad] / nt[bad]}, fp16 floor {floor[bad] / nt[bad]}")
-        # (1) output of the call (prefill returns the last chunk's hidden state) against the exact forward, the bound scaled up
-        #     where this input's fp16 floor is atypically large
-        want, want16 = (res.logits[-1], res16.logits[-1]) if kind == "decode" else (res.hidden, res16.hidden)
-        err, floor = oracle.rel_l2(out[b], want), oracle.rel_l2(want16, want)
-        bound = OUT_TOL[sched] * max(1.0, floor / FLOOR_TYPICAL)
-        floored += bound > OUT_TOL[sched]
-        worst, worst_floor = max(worst, err), max(worst_floor, floor)
-        assert err <= bound, f"{sched} seq {b}: rel-L2 {err:.3e} vs the fp64 truth (bound {bound:.3e}, fp16 floor {floor:.3e})"
+        dt.check_branch(sched, kind, calls, dec, L)
+    worst, worst_floor, floored = dt.check_call(dec, truth, sched, kind, ids, out, pre, dt.snapshot(dec), pos0, chunk)
     print(f"TRUTH {sched} {cfg.name} Q{bits} {kind} B={B} T={T} pos0={pos0}: out rel-L2 {worst:.3e} floor {worst_floor:.3e} "
           f"floored {floored}")
     return worst
@@ -415,7 +227,7 @@ def test_decode_vs_fp64(sched, model, bits, monkeypatch, request):
     dec = _decoder(model, B, bits, fused, chained, row_gemv)
     try:
         truth = _truth_model(dec, SEED)
-        spy = Spy(monkeypatch)
+        spy = dt.Spy(monkeypatch)
         V = dec.cfg.vocab_size
         _call(dec, truth, sched, "prefill", _ids(B, 9, V, 1), spy)
         graph = sched == "D1"
@@ -431,33 +243,9 @@ def test_decode_vs_fp64(sched, model, bits, monkeypatch, request):
 
 
 def _graph_matches_eager(dec, ids, spy):
-    """(4) one step eagerly, then the same step (same cache state) by graph replay: identical logits and cache bytes.  Leaves
-    the decoder as it was, with the graph armed, for the checked call that follows."""
-    c = dec.cache
-    state = [t.clone() for t in (*c.key_states, *c.key_scales, *c.value_states, *c.value_scales, c.cache_seqlens)]
-
-    def restore():
-        for dst, src in zip((*c.key_states, *c.key_scales, *c.value_states, *c.value_scales, c.cache_seqlens), state):
-            dst.copy_(src)
-
-    g, dec.graph = dec.graph, None
-    x = torch.from_numpy(ids).to(DEV)
+    """(4) graph replay produces eager's bits (decoder_truth.graph_matches_eager), the eager step on the D1 branch."""
     spy.take()
-    eager = dec.decode(x).clone()
-    eager_cache = _snapshot(dec)
-    _check_branch("D1", "decode", spy.take(), dec, dec.cfg.num_layers)
-    restore()
-    dec.pos -= 1
-    dec.graph = g
-    replay = dec.decode(x).clone()
-    replay_cache = _snapshot(dec)
-    assert torch.equal(eager.view(torch.int16), replay.view(torch.int16)), "graph replay differs from the eager step"
-    for key in ("k", "ks", "v", "vs"):
-        for a, b in zip(eager_cache[key], replay_cache[key]):
-            assert np.array_equal(a.view(np.uint8), b.view(np.uint8)), f"graph replay stored different {key}"
-    assert np.array_equal(eager_cache["seqlens"], replay_cache["seqlens"])
-    restore()
-    dec.pos -= 1
+    dt.graph_matches_eager(dec, ids, lambda: dt.check_branch("D1", "decode", spy.take(), dec, dec.cfg.num_layers))
 
 
 # ---- prompt schedules -----------------------------------------------------------------------------------------------------
@@ -498,7 +286,7 @@ def test_prompt_vs_fp64(sched, model, bits, monkeypatch, request):
     dec = _decoder(model, B, bits, fused, chained, row_gemv)
     try:
         truth = _truth_model(dec, SEED)
-        spy = Spy(monkeypatch)
+        spy = dt.Spy(monkeypatch)
         for i, T in enumerate(lens):
             if kind == "rows":
                 assert (B * T > 16) == (sched != "P3c")       # P3c: the <= 16-row branch of the blocks
@@ -520,7 +308,7 @@ def test_long_prompt_then_decode_across_a_page(model, bits, monkeypatch, request
     dec = _decoder(model, 1, bits)
     try:
         truth = _truth_model(dec, SEED)
-        spy = Spy(monkeypatch)
+        spy = dt.Spy(monkeypatch)
         V = dec.cfg.vocab_size
         _call(dec, truth, "L", "rows", _ids(1, 252, V, 30), spy)
         for t in range(6):

@@ -7,46 +7,20 @@ gemv_i8_kernel reads a group's scale row and its stage descriptors from shared m
 Here the kernel's request / wait / consume order is replayed over the plans gemv_i8_launch builds (exl2b_debug_i8_plan) for the
 flagship 7B launch structures and the GPTQ and 70B presets: every read must find the entry it expects, delivered by a barrier
 that has already been waited for, and the CTA must fit the 111 KB that keeps two CTAs co-resident per SM."""
-import ctypes
-
 import numpy as np
 import pytest
 
-I8_BARS, I8_LWIN, MAX_REGIONS = 8, 16, 6
+from i8_plans import SMEM_BUDGET, SMEM_LIMIT, ARENA_FLOOR, mat as _mat, plan as _plan_on
+
+I8_BARS, I8_LWIN = 8, 16
 SMS, WARPS = 132, 16
-SMEM_BUDGET = 111 * 1024
-
-
-def _mat(N, KS, regions, gptq=0):
-    """regions: (ks_begin, bits, spg_log2); group_base / off_base derived as qmatrix.cu build_regions does."""
-    reg, gbase, off = [], 0, 0
-    for i, (ks0, bits, lg) in enumerate(regions):
-        ks1 = regions[i + 1][0] if i + 1 < len(regions) else KS
-        reg += [ks0, bits, lg, gbase, off]
-        gbase += -(-(ks1 - ks0) // (1 << lg))
-        off += (ks1 - ks0) * 128 * bits
-    rec = [N, KS, gptq, off, len(regions)] + reg
-    return rec + [0] * (5 + 5 * MAX_REGIONS - len(rec))
 
 
 def _plan(mats, ctas=SMS, warps=WARPS):
-    from exllamav2_b200 import ext as ext_c
-    f = ext_c.lib.exl2b_debug_i8_plan
-    f.restype = ctypes.c_int
-    f.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
-                  ctypes.c_int, ctypes.c_void_p]
-    m = np.asarray(sum(mats, []), dtype=np.int32)
-    units = sum(-(-r[0] // 32) for r in mats) * mats[0][1]
-    cap = units + ctas * warps * 8
-    desc = np.zeros((cap, 4), dtype=np.uint32)
-    first = np.zeros(ctas * warps + 1, dtype=np.uint32)
-    info = np.zeros(6, dtype=np.int32)
-    assert f(m.ctypes.data, len(mats), ctas, warps, desc.ctypes.data, cap, first.ctypes.data, len(first), info.ctypes.data) == 0
-    C, nd = int(info[0]), int(info[1])
-    return desc[:nd], first[: C * warps + 1], C, dict(arena=int(info[2]), srow=int(info[3]), smem=int(info[4]), lcap=int(info[5]))
+    return _plan_on(mats, ctas, warps)
 
 
-K4, K11, K8, K28 = 128, 344, 256, 896          # slabs (32 rows) of K = 4096, 11008, 8192, 28672
+K4, K11, K8, K28, K64 = 128, 344, 256, 896, 2048    # slabs (32 rows) of K = 4096, 11008, 8192, 28672, 65536
 M54_4K = [(0, 5, 2), (13, 4, 2)]
 M54_11K = [(0, 5, 2), (36, 4, 2)]
 M43_4K = [(0, 4, 2), (13, 3, 2)]
@@ -63,7 +37,10 @@ STRUCTURES = {
     "gptq gate|up": [_mat(11008, K4, [(0, 4, 2)], gptq=1)] * 2,
     "gptq down": [_mat(4096, K11, [(0, 4, 2)], gptq=1)],
     # llama2-70b-2.5bpw: g64 MLP (every second slab flushes), the longest stage lists
-    "70b q|k|v": [_mat(8192, K8, [(0, 4, 2), (26, 3, 2)]), _mat(1024, K8, [(0, 4, 2), (26, 3, 2)]), _mat(1024, K8, [(0, 4, 2), (26, 3, 2)])],
+    # (attention [4,3] at 0.1 / 0.9, g128: ceil(819.2 / 128) = 7 groups of 4 bits, 28 slabs)
+    "70b q|k|v": [_mat(8192, K8, [(0, 4, 2), (28, 3, 2)]), _mat(1024, K8, [(0, 4, 2), (28, 3, 2)]), _mat(1024, K8, [(0, 4, 2), (28, 3, 2)])],
+    "70b o": [_mat(8192, K8, [(0, 4, 2), (28, 3, 2)])],
+    "70b head": [_mat(32000, K8, [(0, 6, 2)])],
     "70b gate|up": [_mat(28672, K8, [(0, 3, 1), (78, 2, 1)])] * 2,
     "70b down": [_mat(8192, K28, [(0, 3, 1), (270, 2, 1)])],
     # small cases of the GPU tests: every stage flushes (8-bit g32), groups spanning stages (g256), ragged N
@@ -71,7 +48,12 @@ STRUCTURES = {
     "g256": [_mat(1024, 64, [(0, 4, 3)])],
     "N = 1000": [_mat(1000, 16, [(0, 3, 0), (3, 2, 2)])],
     "K = 16384 8-bit g32": [_mat(4096, 512, [(0, 8, 0)])],
+    # over the budget (test_gpu_full_shapes runs both): the staged row alone is KS * 64 B, so the arenas shrink to the floor and the
+    # CTA still needs more than 111 KB -- it runs one CTA per SM
+    "70b gptq down": [_mat(8192, K28, [(0, 4, 2)], gptq=1)],
+    "K = 65536 4-bit g128": [_mat(1024, K64, [(0, 4, 2)])],
 }
+OVER_BUDGET = {"70b gptq down", "K = 65536 4-bit g128"}
 
 
 def _replay(lst, n_pre):
@@ -129,9 +111,12 @@ def _replay(lst, n_pre):
 def test_smem_operands(name):
     mats = STRUCTURES[name]
     desc, first, C, info = _plan(mats)
-    assert info["smem"] <= SMEM_BUDGET, f"{info['smem']} B of dynamic shared memory"
+    if name in OVER_BUDGET:
+        assert info["arena"] == ARENA_FLOOR and SMEM_BUDGET < info["smem"] <= SMEM_LIMIT, info
+    else:
+        assert info["smem"] <= SMEM_BUDGET, f"{info['smem']} B of dynamic shared memory"
     assert info["srow"] == (128 if any(m[2] for m in mats) else 64)
-    assert info["arena"] >= 2048
+    assert info["arena"] >= ARENA_FLOOR
     n_pre = (first >> 26).astype(int)
     first = (first & 0x3FFFFFF).astype(np.int64)
     longest = 0
