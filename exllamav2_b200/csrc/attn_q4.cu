@@ -110,13 +110,6 @@ __host__ __device__ inline AttnSmem attn_smem_map(int hd, int kb, int vb, int pa
     return m;
 }
 
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-template <int BYTES>
-__device__ __forceinline__ void cp_async_small(uint32_t dst, const void* src) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" ::"r"(dst), "l"(src), "n"(BYTES) : "memory");
-}
 template <bool GLOBAL, typename T>
 __device__ __forceinline__ T ld_rows(const T* p) {      // a cached row: straight from the cache, or from its copy in shared memory
     if constexpr (GLOBAL) return __ldg(p);
@@ -806,6 +799,18 @@ using namespace exl2b;
 
 static int32_t* g_attn_err[64] = {nullptr};
 
+// the sticky status word of `device` that every fused attention kernel sets (exl2b_paged_attn_status), created on first use
+namespace exl2b {
+int attn_err_flag(int device, int32_t** flag) {
+    if (!g_attn_err[device]) {
+        EXL2B_CUDA(cudaMalloc(&g_attn_err[device], sizeof(int32_t)));
+        EXL2B_CUDA(cudaMemset(g_attn_err[device], 0, sizeof(int32_t)));
+    }
+    *flag = g_attn_err[device];
+    return 0;
+}
+}  // namespace exl2b
+
 // Split-KV partial results and arrival counters, one set per (device, stream) like the wgmma workspace (gemv.cu): launches on
 // different streams never merge each other's partials.  Allocated once at the bound every split launch fits in and never
 // freed or moved, because a captured graph keeps the pointers it was captured with.  attn_launch_plan splits only when
@@ -930,11 +935,10 @@ extern "C" int exl2b_paged_attn_decode_q(const uint16_t* q, const uint16_t* k_ne
     const int sms = device_sm_count(dev);
     const AttnLaunch L = attn_launch_plan(kb, vb, head_dim, q_len, num_heads, batch, page_size, pages_per_seq, sms);
     EXL2B_REQUIRE(L.smem.total <= AQ_SMEM_MAX, "context of %d tokens does not fit the score buffer", P.max_ctx);
-    if (!g_attn_err[dev]) {
-        EXL2B_CUDA(cudaMalloc(&g_attn_err[dev], sizeof(int32_t)));
-        EXL2B_CUDA(cudaMemset(g_attn_err[dev], 0, sizeof(int32_t)));
+    {
+        int rc = attn_err_flag(dev, &P.err);
+        if (rc) return rc;
     }
-    P.err = g_attn_err[dev];
     if (L.nsplit > 1) {
         AttnScratch* s = nullptr;
         int rc = attn_scratch(dev, (cudaStream_t)stream, sms, &s);

@@ -91,6 +91,7 @@ _sig("exl2b_qmlp_destroy", c_int, c_void_p)
 _sig("exl2b_qmlp_forward", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p)
 _sig("exl2b_qmlp_forward_gateup", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p)
 _sig("exl2b_paged_attn_decode_q", c_int, *([c_void_p] * 10 + [c_int] * 7 + [c_float, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]))
+_sig("exl2b_paged_attn_prefill_q", c_int, *([c_void_p] * 10 + [c_int] * 7 + [c_float, c_int, c_void_p]))
 _sig("exl2b_paged_attn_status", c_int, c_int, POINTER(c_int))
 _sig("exl2b_paged_attn_clear_status", c_int, c_int)
 _sig("exl2b_debug_scratch", c_int, c_int, c_void_p, c_int, POINTER(c_void_p), POINTER(ctypes.c_size_t))
@@ -583,6 +584,35 @@ def paged_attn_decode_q4(q, k_new, v_new, k_cache, k_scales, v_cache, v_scales, 
         _p(cache_seqlens), _p(block_table), _p(out), B, q_len, H, KVH, hd, k_cache.shape[1], block_table.shape[1],
         float(softmax_scale), out_consumer or None, _p(sin), _p(cos), int(style), sin.shape[-1] if sin is not None else 0,
         int(wbits), _stream(q)))
+
+
+def paged_attn_prefill_q(q, k_new, v_new, k_cache, k_scales, v_cache, v_scales, cache_seqlens, block_table, out,
+                         softmax_scale: float, wbits: int = 4):
+    """Prompt attention over the paged Q4 / Q6 / Q8 cache for any q_len, with quantise-and-append of the new rows (include/
+    exl2_b200.h exl2b_paged_attn_prefill_q).  Shapes as paged_attn_decode_q4; q is RoPE-rotated already.  No reference
+    counterpart as one op: it replaces q_to_fp16_kv + flash_attn_with_kvcache + fp16_to_q_kv (attn.py:560-621)."""
+    B, q_len, H, hd = q.shape
+    KVH = k_new.shape[2]
+    for t in (q, k_new, v_new, out):
+        _dtype(_cuda(t, "attention operand"), torch.half, "attention operand")
+    for t, dt, what in ((k_cache, torch.uint8, "k_cache"), (v_cache, torch.uint8, "v_cache"), (k_scales, torch.half, "k_scales"),
+                        (v_scales, torch.half, "v_scales"), (cache_seqlens, torch.int32, "cache_seqlens"),
+                        (block_table, torch.int32, "block_table")):
+        _dtype(_cuda(t, what), dt, what)
+    _check_kv_shapes(k_new, k_cache, v_new, v_cache, wbits)
+    if tuple(k_new.shape) != (B, q_len, KVH, hd) or tuple(v_new.shape) != (B, q_len, KVH, hd) or tuple(out.shape) != (B, q_len, H, hd):
+        raise RuntimeError(f"k_new / v_new must be [{B}, {q_len}, KVH, {hd}] and out [{B}, {q_len}, {H}, {hd}]; got "
+                           f"{tuple(k_new.shape)}, {tuple(v_new.shape)}, {tuple(out.shape)}")
+    if tuple(k_cache.shape[2:3]) != (KVH,) or k_scales.shape[-1] * 32 != hd or v_scales.shape[-1] * 32 != hd:
+        raise RuntimeError(f"cache tensors must be [pages, page_size, {KVH}, ...] with {hd // 32} scales per row")
+    if block_table.dim() != 2 or cache_seqlens.shape[0] != block_table.shape[0] or block_table.shape[0] != B:
+        raise RuntimeError("cache_seqlens and block_table have incompatible shapes")
+    for t in (q, k_new, v_new, out, k_cache, k_scales, v_cache, v_scales, cache_seqlens, block_table):
+        if not t.is_contiguous():
+            raise RuntimeError("attention operands must be contiguous")
+    _check(lib.exl2b_paged_attn_prefill_q(
+        _p(q), _p(k_new), _p(v_new), _p(k_cache), _p(k_scales), _p(v_cache), _p(v_scales), _p(cache_seqlens), _p(block_table),
+        _p(out), B, q_len, H, KVH, hd, k_cache.shape[1], block_table.shape[1], float(softmax_scale), int(wbits), _stream(q)))
 
 
 def paged_attn_clear_status(device) -> None:

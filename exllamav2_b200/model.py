@@ -413,10 +413,18 @@ class ExLlamaV2Decoder:
             self._forward_tokens(x, q, k, v, ao, n)
         return x
 
-    def prefill_rows(self, ids: torch.Tensor):
+    def prefill_rows(self, ids: torch.Tensor, cache_attn: bool = False):
         """Whole prompt [B, T] in ONE pass per matrix (the many-row path, csrc/gemm_big.cu), in the reference's own op sequence for
         a prompt chunk (attn.py:466-638): get_kv_state -> q_attn_forward_1 -> flash_attn_with_kvcache on the fp16 temp (third-party
-        there too; torch SDPA when flash-attn does not run on this GPU) -> store_kv_state -> q_attn_forward_2 -> q_mlp_forward_."""
+        there too; torch SDPA when flash-attn does not run on this GPU) -> store_kv_state -> q_attn_forward_2 -> q_mlp_forward_.
+
+        cache_attn=True: prompt attention straight over the quantised cache instead (csrc/attn_prefill.cu): q_attn_forward_1 ->
+        paged_attn_prefill_q, which attends and appends the new rows in one launch -> q_attn_forward_2 -> q_mlp_forward_rows.  No
+        fp16 temp, no host synchronisation: the call can be captured in a CUDA graph.  The default stays the reference sequence
+        until the two have been measured against each other on the workloads this decoder serves (tools/bench_prefill_attn.py);
+        making the new path the default is left to that later decision."""
+        if cache_attn:
+            return self._prefill_rows_cache_attn(ids)
         B, T = ids.shape
         cfg, cache = self.cfg, self.cache
         H, KVH, hd = cfg.num_heads, cfg.num_kv_heads, cfg.head_dim
@@ -440,6 +448,30 @@ class ExLlamaV2Decoder:
                 ao = _sdpa_prefill(q.view(B, T, H, hd), k.view(B, T, KVH, hd), v.view(B, T, KVH, hd), tk, tv, cache, hd)
             cache.store_kv_state(li, T)
             ext_c.q_attn_forward_2(L.attn, x, ao.reshape(B, T, H * hd), B, T)
+            ext_c.q_mlp_forward_rows(L.mlp, x.view(B * T, -1), ta, tb)
+        cache.cache_seqlens.add_(T)
+        return x
+
+    def _prefill_rows_cache_attn(self, ids: torch.Tensor):
+        B, T = ids.shape
+        cfg, cache = self.cfg, self.cache
+        H, KVH, hd = cfg.num_heads, cfg.num_kv_heads, cfg.head_dim
+        if self.pos + T > cache.max_seq_len:
+            raise RuntimeError(f"prompt of {T} tokens does not fit the K/V cache")
+        self.pos += T
+        x = self.embed[ids].contiguous()
+        q = torch.empty((B, T, H * hd), dtype=torch.half, device=self.device)
+        k = torch.empty((B, T, KVH * hd), dtype=torch.half, device=self.device)
+        v = torch.empty_like(k)
+        ao = torch.empty_like(q)
+        ta = torch.empty((B * T, cfg.intermediate_size), dtype=torch.half, device=self.device)
+        tb = torch.empty_like(ta)
+        for li, L in enumerate(self.layers):
+            ext_c.q_attn_forward_1(L.attn, x, B, T, -1, cache.cache_seqlens, q, k, v, self.sin, self.cos)
+            ext_c.paged_attn_prefill_q(q.view(B, T, H, hd), k.view(B, T, KVH, hd), v.view(B, T, KVH, hd), cache.key_states[li],
+                                       cache.key_scales[li], cache.value_states[li], cache.value_scales[li], cache.cache_seqlens,
+                                       cache.block_table, ao.view(B, T, H, hd), 1.0 / math.sqrt(hd), wbits=cache.wbits)
+            ext_c.q_attn_forward_2(L.attn, x, ao, B, T)
             ext_c.q_mlp_forward_rows(L.mlp, x.view(B * T, -1), ta, tb)
         cache.cache_seqlens.add_(T)
         return x

@@ -230,6 +230,22 @@ int exl2b_paged_attn_decode_q(const uint16_t* q, const uint16_t* k_new, const ui
                               int num_kv_heads, int head_dim, int page_size, int pages_per_seq, float softmax_scale,
                               exl2b_qmatrix_t out_consumer, const uint16_t* rope_sin, const uint16_t* rope_cos,
                               int rope_style, int sincos_size, int wbits, exl2b_stream_t stream);
+/* Prompt attention straight over the quantised cache, for any q_len >= 1 (replaces the reference's per-layer sequence for a
+ * prompt chunk, q_to_fp16_kv -> flash_attn_with_kvcache -> fp16_to_q_kv, attn.py:560-621 + cache.py:472-556).  Same
+ * semantics as exl2b_paged_attn_decode_q without fused RoPE or a chained output: query i of sequence b sees positions
+ * [0, cache_seqlens[b] + i]; cached positions are the stored values, the q_len new positions are the UNQUANTISED fp16 k_new /
+ * v_new rows (as flash-attn sees them in the reference, before the cache quantises them).  The new rows are quantised with the
+ * fp16_to_q_kv arithmetic and appended at [seqlen, seqlen + q_len): only the new tokens' 64-value units are written, never
+ * widened to 512-value blocks.  Tensor cores (mma.sync m16n8k16, fp16 operands, fp32 accumulation).
+ * Shapes: q [batch,q_len,H,hd] (RoPE applied), k_new / v_new [batch,q_len,KVH,hd], out [batch,q_len,H,hd]; caches and scales as
+ * for exl2b_paged_attn_decode_q; `wbits` 4 / 6 / 8; head_dim 64 or 128; H % KVH == 0; page_size a multiple of 64.
+ * A sequence with cache_seqlens[b] + q_len > pages_per_seq * page_size gets no append and no output, and sets bit 0 of the
+ * status below.  No host synchronisation and no allocation after the first call on a device: the launch can be captured. */
+int exl2b_paged_attn_prefill_q(const uint16_t* q, const uint16_t* k_new, const uint16_t* v_new, uint8_t* k_cache,
+                               uint16_t* k_scales, uint8_t* v_cache, uint16_t* v_scales, const int32_t* cache_seqlens,
+                               const int32_t* block_table, uint16_t* out, int batch, int q_len, int num_heads,
+                               int num_kv_heads, int head_dim, int page_size, int pages_per_seq, float softmax_scale,
+                               int wbits, exl2b_stream_t stream);
 /* Sticky status of the fused attention kernels on `device` (synchronises): bit 0 = a sequence would have run past its page
  * table (cache_seqlens[b] + q_len > pages_per_seq * page_size); that call appended nothing and wrote no output. */
 int exl2b_paged_attn_status(int device, int* status);
