@@ -70,6 +70,7 @@ struct AttnQ4Params {
     unsigned int* cnt;      // [batch][H]
     unsigned long long* dbg;   // optional globaltimer stamps of CTA (dbg_cta, 0, 0) (exl2b_debug_set): 0 start, 1 cache rows requested,
     int dbg_cta;               //   2 dependency wait over, 3 new rows quantised / query rotated, 4 scores + max, 5 P V done; 6 / 7 grid span
+    int pass_len;              // attn_q4_passes_kernel: positions per pass (= sc_len); 0 for attn_q4_kernel
 };
 constexpr int AQ_SPLIT_MIN = 512;
 constexpr int AQ_SUB = 128;            // positions per sub-chunk of the streaming ring (long contexts)
@@ -77,6 +78,15 @@ constexpr int AQ_RING = 4;             // sub-chunks in flight
 constexpr int AQ_STAGE = 512;          // cached positions per CTA staged in shared memory before the dependency wait (Q4; the
                                        // other formats stage the same number of BYTES, host side)
 constexpr int AQ_SMEM_MAX = 200 * 1024;     // dynamic shared memory a launch may use
+// Single-token decode over a cache whose whole-chunk score buffer does not fit AQ_SMEM_MAX walks each CTA's positions in
+// passes (attn_q4_passes_kernel).  The pass length is chosen so that the CTA still shares an SM with one batch-1 GEMV CTA:
+// 228 KB per SM - 111 KB for the GEMV CTA (gemv_i8.cu) - 1 KB reserved per CTA for each of the two - 1 KB for this kernel's
+// static shared memory and slack = 114 KB.  A page table too large for that still runs, with passes of AQ_PASS_MIN positions
+// and without the co-residency; only a page table that leaves no room for AQ_PASS_MIN positions under AQ_SMEM_MAX is refused.
+constexpr int AQ_PASS_SMEM = 114 * 1024;
+constexpr int AQ_PASS_MIN = 512;
+constexpr int AQ_PASS_ALIGN = 256;     // pass lengths are multiples of 256 positions (whole pages at the default page size):
+                                       // a multiple of every ring sub-chunk and score pass
 constexpr int AQ_QPAD = 36;            // floats per 32-value block of the rotated query (bank-staggered: 4 blocks, 4 threads per row)
 constexpr int AQ_QIB = 80;             // bytes per 32-value block of the integer query operands (64 used; bank-staggered like QPAD)
 
@@ -273,8 +283,22 @@ struct AttnCta {
         asm volatile("cp.async.commit_group;" ::: "memory");
         for (int i = tid; i < P.pages_per_seq; i += AQ_THREADS) pages_s[i] = bt[i];
         bt = pages_s;
-        ntail = (P.ring_slots && c_hi > p_lo + n_st) ? (c_hi - (p_lo + n_st) + SUB - 1) / SUB : 0;
+        ntail = ring_chunks();
         return true;
+    }
+    // ring sub-chunks of the cached rows [p_lo + n_st, c_hi) (0 without the ring)
+    __device__ __forceinline__ int ring_chunks() const {
+        return (P.ring_slots && c_hi > p_lo + n_st) ? (c_hi - (p_lo + n_st) + SUB - 1) / SUB : 0;
+    }
+
+    // ---- attn_q4_passes_kernel: the phases below walk [p_lo, n_ctx) with the scores in sc[p - p_lo], the staged window
+    //      [p_lo, p_lo + n_st) and the ring over [p_lo + n_st, c_hi).  Pass [lo, hi) of the CTA's share points them at its
+    //      positions; only the first pass has the staged window (nst), later ones stream every cached row through the ring.
+    __device__ __forceinline__ void begin_pass(int lo, int hi, int nst) {
+        p_lo = lo;
+        c_hi = min(hi, seqlen);
+        n_st = nst;
+        ntail = ring_chunks();
     }
 
     // ---- query i, 64-value unit un, on one warp: qrot = H q * (softmax_scale * log2 e / 32), and its integer operands
@@ -677,11 +701,16 @@ struct AttnCta {
         }
     }
     __device__ __forceinline__ bool end_query(int i, float mx, float denom) const {
+        return end_query(i, mx, denom, [&] { return warp_sum(); });
+    }
+    // the same with the CTA's unnormalised rotated output from `out()` (warps < UNITS) instead of this query's P V sums
+    template <typename F>
+    __device__ __forceinline__ bool end_query(int i, float mx, float denom, F&& out) const {
         if (ns_act > 1) {
             __shared__ int s_last;
             // leave (unnormalised rotated output, max, sum) of this chunk; the last CTA of the (head, sequence) merges them all
             float* wsp = P.ws + (((size_t)b * P.H + h) * P.nsplit + z) * (HD + 2);
-            if (warp < UNITS) __stcg(reinterpret_cast<float2*>(wsp + warp * 64) + lane, warp_sum());
+            if (warp < UNITS) __stcg(reinterpret_cast<float2*>(wsp + warp * 64) + lane, out());
             if (tid == 0) { __stcg(wsp + HD, mx); __stcg(wsp + HD + 1, denom); }
             __threadfence();
             __syncthreads();
@@ -710,7 +739,7 @@ struct AttnCta {
             }
             return false;
         }
-        if (warp < UNITS) store_out(i, warp_sum(), denom);
+        if (warp < UNITS) store_out(i, out(), denom);
         __syncthreads();
         return true;
     }
@@ -758,12 +787,65 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
     cta_exit(P);
 }
 
+// Single-token decode over a cache too long for attn_q4_kernel's score buffer (attn_launch_plan, pass_len): the same phases,
+// run once per pass of at most P.pass_len positions over the CTA's share [p_lo, p_hi) (the whole context, or one split-KV
+// chunk).  Each pass scores, exponentiates against its own max and sums its P V; the CTA carries a running max M, sum L and
+// rotated output across passes, rescaled by exp2(M_old - M_new) -- end_query's split-KV merge, done in sequence -- and hands
+// the final (M, L, output) to end_query.  The staged window belongs to the first pass; every later cached row streams through
+// the ring.  The appended row (position seqlen) is in the last pass of the last chunk.
+template <int HD, int KB, int VB>
+__global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_passes_kernel(const __grid_constant__ AttnQ4Params P) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    EXL2B_STAMP(P, 0);
+    griddep_launch_dependents();
+    if ((int)blockIdx.x >= P.busy_ctas) {
+        if (threadIdx.x == 0) slot_hold(P.slot_cnt, P.busy_ctas);
+        return;
+    }
+    AttnCta<HD, KB, VB> c(P, smem);
+    if (!c.prologue()) return cta_exit(P);
+    EXL2B_STAMP(P, 1);
+    griddep_wait();
+    EXL2B_STAMP(P, 2);
+    c.new_rows_and_first_query();
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    __syncthreads();
+    EXL2B_STAMP(P, 3);
+    // the running output, elements warp * 64 + 2 lane, +1 on warps < UNITS, each read and written by its own thread only.  It
+    // lives in new_y's second key row, which a single query leaves unused (registers would spill at Q4 hd 128).
+    float2* o = reinterpret_cast<float2*>(c.new_y + HD) + c.warp * 32 + c.lane;
+    if (c.warp < c.UNITS) *o = make_float2(0.f, 0.f);
+    float M = -INFINITY, L = 0.f;
+    for (int pl = c.p_lo, nst = c.n_st; pl < c.p_hi; pl += P.pass_len, nst = 0) {
+        const int ph = min(c.p_hi, pl + P.pass_len);
+        c.begin_pass(pl, ph, nst);
+        const float lmax = c.scores(ph);
+        float mx, denom;
+        c.softmax(lmax, ph, mx, denom);
+        c.pv(ph);
+        __syncthreads();
+        const float mn = fmaxf(M, mx), a = exp2f(M - mn), w = exp2f(mx - mn);
+        if (c.warp < c.UNITS) {
+            const float2 s = c.warp_sum(), r = *o;
+            *o = make_float2(fmaf(w, s.x, r.x * a), fmaf(w, s.y, r.y * a));
+        }
+        L = fmaf(w, denom, L * a);
+        M = mn;
+    }
+    EXL2B_STAMP(P, 5);
+    if (c.warp == AQ_WARPS - 1 && c.h % c.group == 0 && c.z == 0) c.append();
+    if (!c.end_query(0, M, L, [&] { return *o; })) return cta_exit(P);
+    if (P.dbg && threadIdx.x == 0) atomicMax(P.dbg + 7, globaltimer());
+    cta_exit(P);
+}
+
 // The launch of one call, from the shape and the SM count alone (tests/attn_regimes.py restates it)
 struct AttnLaunch {
     int nsplit;          // CTAs per (head, sequence)
     int sc_len;          // floats of the score buffer
     int ring_slots;      // AQ_RING with the ring, else 0
     int stage;           // staged cached positions per CTA
+    int pass_len;        // > 0: attn_q4_passes_kernel with passes of this many positions (= sc_len); 0: attn_q4_kernel
     AttnSmem smem;
 };
 static AttnLaunch attn_launch_plan(int kb, int vb, int hd, int q_len, int num_heads, int batch, int page_size, int pages_per_seq,
@@ -790,6 +872,17 @@ static AttnLaunch attn_launch_plan(int kb, int vb, int hd, int q_len, int num_he
     const int window = L.ring_slots ? AQ_STAGE / 2 : AQ_STAGE;
     L.stage = (int)((size_t)window * (hd + 4 * nsc) / (size_t)(rowk + rowv + 4 * nsc)) / 64 * 64;
     L.smem = attn_smem_map(hd, kb, vb, pages_per_seq, L.sc_len, L.stage, L.ring_slots != 0);
+    // A single query whose score buffer does not fit walks its positions in passes instead.  Its buffer then holds one pass,
+    // as long as keeps the CTA within AQ_PASS_SMEM, in multiples of AQ_PASS_ALIGN, at least AQ_PASS_MIN.  (The ring is on: a score buffer of
+    // ~29 000 positions or more means a cache far above 8192.)  Launches that fit keep the plan above.
+    L.pass_len = 0;
+    if (q_len == 1 && L.smem.total > (uint32_t)AQ_SMEM_MAX) {
+        const uint32_t rest = attn_smem_map(hd, kb, vb, pages_per_seq, 0, L.stage, true).total;
+        const int room = rest < (uint32_t)AQ_PASS_SMEM ? (int)((AQ_PASS_SMEM - rest) / 4) : 0;
+        L.pass_len = std::max(AQ_PASS_MIN, room / AQ_PASS_ALIGN * AQ_PASS_ALIGN);
+        L.sc_len = L.pass_len;
+        L.smem = attn_smem_map(hd, kb, vb, pages_per_seq, L.sc_len, L.stage, true);
+    }
     return L;
 }
 
@@ -878,6 +971,13 @@ extern "C" int exl2b_paged_attn_clear_status(int device) {
 
 template <int KB, int VB>
 static int attn_q_launch(int head_dim, dim3 grid, size_t smem, cudaStream_t stream, const AttnQ4Params& P) {
+    if (P.pass_len) {
+        if (head_dim == 128)
+            EXL2B_CUDA(launch_pdl_f("attn", attn_q4_passes_kernel<128, KB, VB>, grid, dim3(AQ_THREADS), smem, stream, P));
+        else
+            EXL2B_CUDA(launch_pdl_f("attn", attn_q4_passes_kernel<64, KB, VB>, grid, dim3(AQ_THREADS), smem, stream, P));
+        return 0;
+    }
     if (head_dim == 128)
         EXL2B_CUDA(launch_pdl_f("attn", attn_q4_kernel<128, KB, VB>, grid, dim3(AQ_THREADS), smem, stream, P));
     else
@@ -889,6 +989,8 @@ template <int KB, int VB>
 static int attn_q_set_smem() {
     EXL2B_CUDA(cudaFuncSetAttribute(attn_q4_kernel<128, KB, VB>, cudaFuncAttributeMaxDynamicSharedMemorySize, AQ_SMEM_MAX));
     EXL2B_CUDA(cudaFuncSetAttribute(attn_q4_kernel<64, KB, VB>, cudaFuncAttributeMaxDynamicSharedMemorySize, AQ_SMEM_MAX));
+    EXL2B_CUDA(cudaFuncSetAttribute(attn_q4_passes_kernel<128, KB, VB>, cudaFuncAttributeMaxDynamicSharedMemorySize, AQ_SMEM_MAX));
+    EXL2B_CUDA(cudaFuncSetAttribute(attn_q4_passes_kernel<64, KB, VB>, cudaFuncAttributeMaxDynamicSharedMemorySize, AQ_SMEM_MAX));
     return 0;
 }
 
@@ -934,6 +1036,10 @@ extern "C" int exl2b_paged_attn_decode_q(const uint16_t* q, const uint16_t* k_ne
     EXL2B_REQUIRE(dev >= 0 && dev < 64, "bad device");
     const int sms = device_sm_count(dev);
     const AttnLaunch L = attn_launch_plan(kb, vb, head_dim, q_len, num_heads, batch, page_size, pages_per_seq, sms);
+    if (L.pass_len)
+        EXL2B_REQUIRE(L.smem.total <= AQ_SMEM_MAX,
+                      "a page table of %d pages needs %u bytes of shared memory with passes of %d positions, above %d",
+                      pages_per_seq, L.smem.total, L.pass_len, AQ_SMEM_MAX);
     EXL2B_REQUIRE(L.smem.total <= AQ_SMEM_MAX, "context of %d tokens does not fit the score buffer", P.max_ctx);
     {
         int rc = attn_err_flag(dev, &P.err);
@@ -954,6 +1060,7 @@ extern "C" int exl2b_paged_attn_decode_q(const uint16_t* q, const uint16_t* k_ne
     P.sc_len = L.sc_len;
     P.ring_slots = L.ring_slots;
     P.stage = L.stage;
+    P.pass_len = L.pass_len;
     P.dbg = exl2b::g_dbg ? exl2b::g_dbg + 32 * (exl2b::g_dbg_slot++ % 64) : nullptr;
     P.dbg_cta = 0;
     static bool attr_set[64] = {false};

@@ -223,7 +223,12 @@ int exl2b_paged_attn_decode(const uint16_t* q, const uint16_t* k_new, const uint
  * none).  Needs sincos_size == head_dim.
  * `out_consumer` (or NULL): the matrix that takes the attention output (o_proj); the output is also left in its activation
  * buffer (chained launches, below) -- as a plain fp16 row in its stored-row order when there is a single row, where the
- * batch-1 GEMV reads it. */
+ * batch-1 GEMV reads it.
+ * Cache length: with q_len 2..8 every CTA holds one fp32 score per position of its share of the cache's capacity
+ * (pages_per_seq * page_size) in shared memory, so capacities above ~29 000 positions (hd 128) are refused ("context of N
+ * tokens does not fit the score buffer").  A single-token step (q_len 1) whose scores do not fit walks each CTA's positions
+ * in passes with an online softmax instead, and is refused only when the page table itself leaves no room for a pass of 512
+ * positions (about 28 600 pages at Q4 hd 128), with an error naming the pages and the bytes (DESIGN.md §3.4). */
 int exl2b_paged_attn_decode_q(const uint16_t* q, const uint16_t* k_new, const uint16_t* v_new, uint8_t* k_cache,
                               uint16_t* k_scales, uint8_t* v_cache, uint16_t* v_scales, const int32_t* cache_seqlens,
                               const int32_t* block_table, uint16_t* out, int batch, int q_len, int num_heads,
