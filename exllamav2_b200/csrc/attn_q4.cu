@@ -69,7 +69,8 @@ struct AttnQ4Params {
     float* ws;              // [batch][H][nsplit][hd + 2]
     unsigned int* cnt;      // [batch][H]
     unsigned long long* dbg;   // optional globaltimer stamps of CTA (dbg_cta, 0, 0) (exl2b_debug_set): 0 start, 1 cache rows requested,
-    int dbg_cta;               //   2 dependency wait over, 3 new rows quantised / query rotated, 4 scores + max, 5 P V done; 6 / 7 grid span
+    int dbg_cta;               //   2 dependency wait over, 3 new rows quantised / query rotated, 4 scores + max, 5 P V done; 6 / 7 grid span;
+                               //   dbg[10] counts the CTAs that took staged_pass (all_staged)
     int pass_len;              // attn_q4_passes_kernel: positions per pass (= sc_len); 0 for attn_q4_kernel
 };
 constexpr int AQ_SPLIT_MIN = 512;
@@ -126,37 +127,40 @@ __device__ __forceinline__ T ld_rows(const T* p) {      // a cached row: straigh
     else return *p;
 }
 
-// one half2 (elements un*64 + 2*lane, +1) of a head row, rotated if RoPE is fused.  Warp-uniform call.
+// the sin / cos pair that rotates one lane's half2 of 64-value unit `un` of a head row at position pos (fused RoPE)
+struct RopeCs {
+    half2 c, s;
+};
 template <int HD>
-__device__ __forceinline__ half2 load_roped(const half* __restrict__ row, int un, int lane, const AttnQ4Params& P, int pos) {
+__device__ __forceinline__ RopeCs rope_cs(int un, int lane, const AttnQ4Params& P, int pos) {
+    // NeoX pairs element j with j + HD / 2: HD == 128, the other unit at the same lane; HD == 64, lane ^ 16
+    const int col = !P.rope_neox ? un * 64 + 2 * lane : HD == 128 ? 2 * lane : 2 * (lane & 15);
+    return {*reinterpret_cast<const half2*>(P.rope_cos + (size_t)pos * P.sincos_size + col),
+            *reinterpret_cast<const half2*>(P.rope_sin + (size_t)pos * P.sincos_size + col)};
+}
+
+// one half2 (elements un*64 + 2*lane, +1) of a head row, rotated with `cs` (rope_cs) if RoPE is fused.  Warp-uniform call.
+template <int HD>
+__device__ __forceinline__ half2 load_roped(const half* __restrict__ row, int un, int lane, const AttnQ4Params& P, const RopeCs& cs) {
     const half2 v = reinterpret_cast<const half2*>(row + un * 64)[lane];
     if (!P.rope_sin) return v;
-    const half* sr = P.rope_sin + (size_t)pos * P.sincos_size;
-    const half* cr = P.rope_cos + (size_t)pos * P.sincos_size;
     if (P.rope_neox) {
         half2 o;
-        int col;
         bool first;
         if constexpr (HD == 128) {            // partner element j + 64 lives in the other 64-value unit, same lane
             o = reinterpret_cast<const half2*>(row + (un ^ 1) * 64)[lane];
-            col = 2 * lane;
             first = (un == 0);
         } else {                              // HD == 64: partner j + 32 is lane ^ 16
             o = __shfl_xor_sync(0xffffffffu, v, 16);
-            col = 2 * (lane & 15);
             first = lane < 16;
         }
-        const half2 c2 = *reinterpret_cast<const half2*>(cr + col);
-        const half2 s2 = *reinterpret_cast<const half2*>(sr + col);
-        if (first) return __hfma2(v, c2, __hmul2(o, __hneg2(s2)));      // l' = l c + half(r * -s)
-        return __hfma2(v, c2, __hmul2(o, s2));                            // r' = r c + half(l * s)
+        if (first) return __hfma2(v, cs.c, __hmul2(o, __hneg2(cs.s)));      // l' = l c + half(r * -s)
+        return __hfma2(v, cs.c, __hmul2(o, cs.s));                            // r' = r c + half(l * s)
     }
-    const int col = un * 64 + 2 * lane;
-    const half2 c01 = *reinterpret_cast<const half2*>(cr + col);
-    half2 s01 = *reinterpret_cast<const half2*>(sr + col);
+    half2 s01 = cs.s;
     uint32_t sb = *reinterpret_cast<uint32_t*>(&s01) ^ (1u << 15);        // (-sin[i], +sin[i+1])
     s01 = *reinterpret_cast<half2*>(&sb);
-    return __hfma2(__lowhigh2highlow(v), s01, __hmul2(v, c01));
+    return __hfma2(__lowhigh2highlow(v), s01, __hmul2(v, cs.c));
 }
 
 // (nibble - 8) as fp32 without I2F: 0x4B000000 | n is the float 2^23 + n
@@ -204,6 +208,7 @@ struct AttnCta {
     int h, b, z, tid, warp, lane, group, kvh, kblk, krow;
     int seqlen, ns_act, p_lo, p_hi, c_hi, n_st, ntail;
     const int* bt;                                 // the sequence's page table: global until the prologue has copied it
+    RopeCs cs0;                                    // fused RoPE: sin / cos at position seqlen of this warp's rope_unit() (load_static)
 
     __device__ __forceinline__ AttnCta(const AttnQ4Params& P_, uint8_t* smem) : P(P_) {
         const AttnSmem m = attn_smem_map(HD, KB, VB, P.pages_per_seq, P.sc_len, P.stage, true);
@@ -286,6 +291,24 @@ struct AttnCta {
         ntail = ring_chunks();
         return true;
     }
+    // operands of the phases after the dependency wait that the Q|K|V launch does not write, fetched just before the wait
+    // (not in the prologue: registers held across staged_pass's first run spill).  The fused-RoPE sin / cos pair is loaded;
+    // the o_proj rows store_out writes are only prefetched into L2, so that they hold no register until the store.
+    __device__ __forceinline__ void load_static() {
+        cs0 = P.rope_sin ? rope_cs<HD>(rope_unit(), lane, P, seqlen) : RopeCs{};
+        if (P.out_invperm && warp < UNITS && lane == 0)
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(P.out_invperm + h * HD + warp * 64));
+    }
+    // the 64-value unit whose RoPE the warp applies first (new_rows_and_first_query): the last UNITS warps rotate the query,
+    // the first ones quantise the new rows, job = warp (key rows are jobs 0 .. UNITS - 1)
+    __device__ __forceinline__ int rope_unit() const {
+        return warp >= AQ_WARPS - UNITS ? warp - (AQ_WARPS - UNITS) : warp % UNITS;
+    }
+    // unit un of a head row at position seqlen + i, rotated if RoPE is fused (sin / cos from the prologue where they match)
+    __device__ __forceinline__ half2 roped(const half* row, int un, int i) const {
+        const bool pre = !P.rope_sin || (i == 0 && un == rope_unit());
+        return load_roped<HD>(row, un, lane, P, pre ? cs0 : rope_cs<HD>(un, lane, P, seqlen + i));
+    }
     // ring sub-chunks of the cached rows [p_lo + n_st, c_hi) (0 without the ring)
     __device__ __forceinline__ int ring_chunks() const {
         return (P.ring_slots && c_hi > p_lo + n_st) ? (c_hi - (p_lo + n_st) + SUB - 1) / SUB : 0;
@@ -303,7 +326,7 @@ struct AttnCta {
 
     // ---- query i, 64-value unit un, on one warp: qrot = H q * (softmax_scale * log2 e / 32), and its integer operands
     __device__ __forceinline__ void rotate_q(int i, int un) {
-        const half2 qh = load_roped<HD>(P.q + (((size_t)b * P.q_len + i) * P.H + h) * HD, un, lane, P, seqlen + i);
+        const half2 qh = roped(P.q + (((size_t)b * P.q_len + i) * P.H + h) * HD, un, i);
         float2 w = hadamard32_f(__half22float2(qh), lane);
         const float f = P.scale_log2 * (1.0f / 32.0f);
         const int e = un * 64 + 2 * lane;
@@ -357,7 +380,7 @@ struct AttnCta {
             const int kv = job / (P.q_len * UNITS), r = job - kv * P.q_len * UNITS;
             const int i = r / UNITS, un = r - i * UNITS;
             const half* src = (kv ? P.v_new : P.k_new) + (((size_t)b * P.q_len + i) * P.KVH + kvh) * HD;
-            half2 w2 = kv ? reinterpret_cast<const half2*>(src + un * 64)[lane] : load_roped<HD>(src, un, lane, P, seqlen + i);
+            half2 w2 = kv ? reinterpret_cast<const half2*>(src + un * 64)[lane] : roped(src, un, i);
             {
                 const float2 y = hadamard32_f(__half22float2(w2), lane);
                 new_y[(kv * AQ_MAX_QLEN + i) * HD + un * 64 + 2 * lane] = y.x;
@@ -471,27 +494,26 @@ struct AttnCta {
         return __half2float(__ushort_as_half((unsigned short)k.s)) * qscl[kblk] * (float)v;
     }
 
+    // this thread's block of the score of new row i (appended by this step): fp16 values, rotated in fp32
+    __device__ __forceinline__ float score_new(int i) const {
+        const float4* y4 = reinterpret_cast<const float4*>(new_y + i * HD + kblk * 32);
+        const float4* q4 = reinterpret_cast<const float4*>(qrot + kblk * AQ_QPAD);
+        float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float4 a = q4[j], c = y4[j];
+            s0 = fmaf(a.x, c.x, s0);
+            s1 = fmaf(a.y, c.y, s1);
+            s2 = fmaf(a.z, c.z, s2);
+            s3 = fmaf(a.w, c.w, s3);
+        }
+        return (s0 + s1) + (s2 + s3);
+    }
+
     // score of position p (warp-uniform call: the NSC partial sums meet by shuffle) into sc[] and the running max
     __device__ __forceinline__ void score_pos(int p, const KeyBlock& k, int n_ctx, float& lmax) const {
         float s = 0.f;
-        if (p < n_ctx) {
-            if (p >= seqlen) {               // a row appended by this step: fp16 values, rotated in fp32
-                const float4* y4 = reinterpret_cast<const float4*>(new_y + (p - seqlen) * HD + kblk * 32);
-                const float4* q4 = reinterpret_cast<const float4*>(qrot + kblk * AQ_QPAD);
-                float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const float4 a = q4[j], c = y4[j];
-                    s0 = fmaf(a.x, c.x, s0);
-                    s1 = fmaf(a.y, c.y, s1);
-                    s2 = fmaf(a.z, c.z, s2);
-                    s3 = fmaf(a.w, c.w, s3);
-                }
-                s = (s0 + s1) + (s2 + s3);
-            } else {
-                s = score_blk(k);
-            }
-        }
+        if (p < n_ctx) s = p >= seqlen ? score_new(p - seqlen) : score_blk(k);
 #pragma unroll
         for (int o = 1; o < TPR; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
         if (p < n_ctx) {
@@ -654,6 +676,80 @@ struct AttnCta {
         for (int j = 0; j < VEC; ++j) red[warp * HD + lane * VEC + j] = acc[j];
     }
 
+    // ---- single query, every cached row of the CTA in the staged window (CTA-uniform): staged_pass instead of scores /
+    //      softmax / pv
+    __device__ __forceinline__ bool all_staged() const { return P.q_len == 1 && ntail == 0 && c_hi - p_lo <= n_st; }
+    // Each warp attends a contiguous range of the CTA's positions [p_lo, p_hi) (the appended row included, where it falls) on
+    // its own: G positions per step scored as in scores() (TPR lanes each), a running max m and sum l, P V accumulated in
+    // pv()'s layout with each weight shuffled from its position's lanes -- no score buffer, no barrier.  One barrier, then the
+    // warps' (m, l, output) merge in warp order with weights exp2(m_w - M), end_query's split-KV merge, into (M, L, w) on
+    // warps < UNITS (the triple end_query takes).  Reads only shared memory and writes only red / wred: it may also run on
+    // whatever shared memory holds, with its results discarded (attn_q4_kernel runs it once before the dependency wait).
+    __device__ __forceinline__ void staged_pass(float& M, float& L, float2& w) const {
+        constexpr int G = 32 / TPR;
+        const int per = (p_hi - p_lo + AQ_WARPS * G - 1) / (AQ_WARPS * G) * G;      // whole steps per warp
+        const int lo = p_lo + warp * per, hi = min(p_hi, lo + per), c_end = min(hi, seqlen);
+        const float* y_new = new_y + AQ_MAX_QLEN * HD + lane * VEC;                 // the appended value row, this lane's part
+        float m = -INFINITY, l = 0.f, acc[VEC];
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) acc[j] = 0.f;
+        for (int pb = lo; pb < hi; pb += G) {
+            const int pp = pb + lane / TPR;
+            float s = 0.f;
+            if (pp < c_end) s = score_blk(key_block<false>(kst + (pp - p_lo) * ROWBK, ksst + (pp - p_lo) * NSC));
+            else if (pp < hi) s = score_new(0);
+#pragma unroll
+            for (int o = 1; o < TPR; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            if (pp >= hi) s = -INFINITY;
+            float mn = s;
+#pragma unroll
+            for (int o = TPR; o < 32; o <<= 1) mn = fmaxf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+            mn = fmaxf(m, mn);                                   // finite: position pb is in range
+            const float a = exp2f(m - mn), e = exp2f(s - mn);
+            m = mn;
+            l = fmaf(l, a, kblk == 0 ? e : 0.f);                 // each position counted on its first lane
+#pragma unroll
+            for (int j = 0; j < VEC; ++j) acc[j] *= a;
+#pragma unroll 2
+            for (int r = 0; r < G; ++r) {
+                const int p = pb + r;
+                const float pw = __shfl_sync(0xffffffffu, e, r * TPR);
+                if (p < c_end) {
+                    pv_fma(acc, value_row<false>(vst + (p - p_lo) * ROWBV, vsst + (p - p_lo) * NSC), pw);
+                } else if (p < hi) {
+#pragma unroll
+                    for (int j = 0; j < VEC; ++j) acc[j] = fmaf(pw, y_new[j], acc[j]);
+                }
+            }
+        }
+#pragma unroll
+        for (int o = TPR; o < 32; o <<= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) red[warp * HD + lane * VEC + j] = acc[j];
+        if (lane == 0) {
+            wred[warp] = m;
+            wred[AQ_WARPS + warp] = l;
+        }
+        EXL2B_STAMP(P, 4);
+        __syncthreads();
+        EXL2B_STAMP(P, 5);
+        M = -INFINITY;
+        L = 0.f;
+        w = make_float2(0.f, 0.f);
+        if (warp < UNITS) {          // elements warp * 64 + 2 lane, +1 of the rotated output (a warp with no positions weighs 0)
+#pragma unroll
+            for (int ww = 0; ww < AQ_WARPS; ++ww) M = fmaxf(M, wred[ww]);
+#pragma unroll
+            for (int ww = 0; ww < AQ_WARPS; ++ww) {
+                const float wgt = exp2f(wred[ww] - M);
+                const float2 a = reinterpret_cast<const float2*>(red + ww * HD + warp * 64)[lane];
+                w.x = fmaf(wgt, a.x, w.x);
+                w.y = fmaf(wgt, a.y, w.y);
+                L = fmaf(wgt, wred[AQ_WARPS + ww], L);
+            }
+        }
+    }
+
     // ---- the rows appended by this step go to the cache, from shared memory, on one warp
     __device__ __forceinline__ void append() const {
         constexpr int WK = ROWBK / 4, WV = ROWBV / 4;                 // 32-bit words per key / value row
@@ -740,7 +836,7 @@ struct AttnCta {
             return false;
         }
         if (warp < UNITS) store_out(i, out(), denom);
-        __syncthreads();
+        if (i + 1 < P.q_len) __syncthreads();      // the next query reuses the shared buffers; after the last, the CTA leaves
         return true;
     }
 };
@@ -759,29 +855,52 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
     // q / k_new / v_new arrive
     if (!c.prologue()) return cta_exit(P);
     EXL2B_STAMP(P, 1);
-    griddep_wait();
-    EXL2B_STAMP(P, 2);
-    c.new_rows_and_first_query();
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    __syncthreads();
-    EXL2B_STAMP(P, 3);
-    EXL2B_STAMP(P, 8);
-    for (int i = 0; i < P.q_len; ++i) {
-        const int n_ctx = (P.nsplit > 1) ? c.p_hi : c.seqlen + i + 1;          // end of the positions this CTA attends for query i
-        if (i > 0) {                         // (the first query was rotated above, next to the quantisation)
-            if (c.warp < c.UNITS) c.rotate_q(i, c.warp);
-            __syncthreads();
-        }
-        const float lmax = c.scores(n_ctx);
-        EXL2B_STAMP(P, 9);
-        float mx, denom;
-        c.softmax(lmax, n_ctx, mx, denom);
-        c.pv(n_ctx);
+    const auto after_wait = [&] {
+        c.load_static();
+        griddep_wait();
+        EXL2B_STAMP(P, 2);
+        c.new_rows_and_first_query();
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
         __syncthreads();
-        EXL2B_STAMP(P, 5);
+        EXL2B_STAMP(P, 3);
+        EXL2B_STAMP(P, 8);
+    };
+    if (c.all_staged()) {
+        // The warp-local pass (staged_pass) runs twice from ONE copy of its code: first before the dependency wait, on whatever
+        // shared memory holds, its results discarded; then for real.  The first run costs nothing on the critical path (the
+        // CTA waits for the Q|K|V launch anyway) and leaves the pass's instructions in this SM's instruction cache: the GEMV
+        // launches stream ~100 MB of weights through the 50 MB L2 per layer, so without it every line of the pass is
+        // fetched from HBM after the wait.
+        float M = 0.f, L = 0.f;
+        float2 w = make_float2(0.f, 0.f);
+#pragma unroll 1
+        for (int round = HD == 128 ? 0 : 1; round < 2; ++round) {      // (at HD 64 the first run spills: not done)
+            if (round == 1) after_wait();
+            c.staged_pass(M, L, w);
+        }
+        if (P.dbg && threadIdx.x == 0) atomicAdd(P.dbg + 10, 1ull);
         // the last warp appends (it has no part in the end of the query): nothing on the way to the output waits for these stores
-        if (i == P.q_len - 1 && c.warp == AQ_WARPS - 1 && c.h % c.group == 0 && c.z == 0) c.append();
-        if (!c.end_query(i, mx, denom)) return cta_exit(P);
+        if (c.warp == AQ_WARPS - 1 && c.h % c.group == 0 && c.z == 0) c.append();
+        if (!c.end_query(0, M, L, [&] { return w; })) return cta_exit(P);
+    } else {
+        after_wait();
+        for (int i = 0; i < P.q_len; ++i) {
+            const int n_ctx = (P.nsplit > 1) ? c.p_hi : c.seqlen + i + 1;          // end of the positions this CTA attends for query i
+            if (i > 0) {                         // (the first query was rotated above, next to the quantisation)
+                if (c.warp < c.UNITS) c.rotate_q(i, c.warp);
+                __syncthreads();
+            }
+            const float lmax = c.scores(n_ctx);
+            EXL2B_STAMP(P, 9);
+            float mx, denom;
+            c.softmax(lmax, n_ctx, mx, denom);
+            c.pv(n_ctx);
+            __syncthreads();
+            EXL2B_STAMP(P, 5);
+            // the last warp appends (it has no part in the end of the query): nothing on the way to the output waits for these stores
+            if (i == P.q_len - 1 && c.warp == AQ_WARPS - 1 && c.h % c.group == 0 && c.z == 0) c.append();
+            if (!c.end_query(i, mx, denom)) return cta_exit(P);
+        }
     }
     if (P.dbg && threadIdx.x == 0) atomicMax(P.dbg + 7, globaltimer());
     cta_exit(P);
@@ -805,6 +924,7 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_passes_kernel(const __g
     AttnCta<HD, KB, VB> c(P, smem);
     if (!c.prologue()) return cta_exit(P);
     EXL2B_STAMP(P, 1);
+    c.load_static();
     griddep_wait();
     EXL2B_STAMP(P, 2);
     c.new_rows_and_first_query();
