@@ -121,9 +121,12 @@ __host__ __device__ inline AttnSmem attn_smem_map(int hd, int kb, int vb, int pa
     return m;
 }
 
+// A cached row: straight from the cache, or from its copy in shared memory.  Cached K/V rows and their scales are read once per
+// step (every copy and load of them below is evict-first in L2, common.cuh); the rows this step appends, the page table,
+// sin / cos, q / k / v and the split-KV scratch keep the default policy.
 template <bool GLOBAL, typename T>
-__device__ __forceinline__ T ld_rows(const T* p) {      // a cached row: straight from the cache, or from its copy in shared memory
-    if constexpr (GLOBAL) return __ldg(p);
+__device__ __forceinline__ T ld_rows(const T* p) {
+    if constexpr (GLOBAL) return ldg_ef(p);
     else return *p;
 }
 
@@ -277,13 +280,13 @@ struct AttnCta {
         for (int idx = tid; idx < n_st * CH; idx += AQ_THREADS) {
             const int pos = idx / CH, ch = idx - pos * CH;
             const size_t r = row(p_lo + pos);
-            if (ch < CHK) cp_async16(smem_addr(kst + pos * ROWBK + ch * 16), P.k_q + r * ROWBK + ch * 16);
-            if (ch < CHV) cp_async16(smem_addr(vst + pos * ROWBV + ch * 16), P.v_q + r * ROWBV + ch * 16);
+            if (ch < CHK) cp_async16_ef(smem_addr(kst + pos * ROWBK + ch * 16), P.k_q + r * ROWBK + ch * 16);
+            if (ch < CHV) cp_async16_ef(smem_addr(vst + pos * ROWBV + ch * 16), P.v_q + r * ROWBV + ch * 16);
         }
         for (int pos = tid; pos < n_st; pos += AQ_THREADS) {
             const size_t r = row(p_lo + pos);
-            cp_async_small<NSC * 2>(smem_addr(ksst + pos * NSC), P.k_s + r * NSC);
-            cp_async_small<NSC * 2>(smem_addr(vsst + pos * NSC), P.v_s + r * NSC);
+            cp_async_small_ef<NSC * 2>(smem_addr(ksst + pos * NSC), P.k_s + r * NSC);
+            cp_async_small_ef<NSC * 2>(smem_addr(vsst + pos * NSC), P.v_s + r * NSC);
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
         for (int i = tid; i < P.pages_per_seq; i += AQ_THREADS) pages_s[i] = bt[i];
@@ -409,10 +412,10 @@ struct AttnCta {
         const int base = p_lo + n_st + t * SUB, cnt = min(SUB, c_hi - base), slot = t & (AQ_RING - 1);
         for (int idx = tid; idx < cnt * CH; idx += AQ_THREADS) {
             const int pos = idx / CH, ch = idx - pos * CH;
-            cp_async16(smem_addr(rq + (slot * SUB + pos) * ROWB + ch * 16), gq + row(base + pos) * RB + ch * 16);
+            cp_async16_ef(smem_addr(rq + (slot * SUB + pos) * ROWB + ch * 16), gq + row(base + pos) * RB + ch * 16);
         }
         for (int pos = tid; pos < cnt; pos += AQ_THREADS)
-            cp_async_small<NSC * 2>(smem_addr(rs + (slot * SUB + pos) * NSC), gs + row(base + pos) * NSC);
+            cp_async_small_ef<NSC * 2>(smem_addr(rs + (slot * SUB + pos) * NSC), gs + row(base + pos) * NSC);
         asm volatile("cp.async.commit_group;" ::: "memory");
     }
     // long context: the cached rows beyond the staged window stream through the ring, AQ_RING sub-chunks in flight;
@@ -868,9 +871,9 @@ __global__ void __launch_bounds__(AQ_THREADS, 2) attn_q4_kernel(const __grid_con
     if (c.all_staged()) {
         // The warp-local pass (staged_pass) runs twice from ONE copy of its code: first before the dependency wait, on whatever
         // shared memory holds, its results discarded; then for real.  The first run costs nothing on the critical path (the
-        // CTA waits for the Q|K|V launch anyway) and leaves the pass's instructions in this SM's instruction cache: the GEMV
-        // launches stream ~100 MB of weights through the 50 MB L2 per layer, so without it every line of the pass is
-        // fetched from HBM after the wait.
+        // CTA waits for the Q|K|V launch anyway) and leaves the pass's instructions in this SM's instruction cache.  The
+        // evict-first policy of the weight and cache streams (common.cuh) does not make this run redundant: without it the
+        // pass takes ~4.4 us after the wait, with it ~2.6 us (DESIGN §7).
         float M = 0.f, L = 0.f;
         float2 w = make_float2(0.f, 0.f);
 #pragma unroll 1

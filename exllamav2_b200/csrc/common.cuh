@@ -151,6 +151,51 @@ __device__ __forceinline__ void cp_async_small(uint32_t dst, const void* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" ::"r"(dst), "l"(src), "n"(BYTES) : "memory");
 }
 
+// ---- L2 eviction priority of data a decode step reads exactly once: the weights and the cached K/V rows.  A step streams
+//      ~3.3 GB of them through the 50 MB L2; at normal priority they push out what every launch reuses (kernel code, launch
+//      plans, norm weights, permutations, sin / cos, the rows one launch leaves for the next).  Loads and copies of such data
+//      use the `_ef` variants below (evict-first); everything else keeps the unhinted helpers.
+// Each variant makes its policy where it is used: a policy hoisted into a register and held across a loop costs the
+// attention kernels, which sit at their 128-register cap, spills; made at each use (volatile, so it is not hoisted) it costs one
+// instruction per copy and no register beyond the copy.
+__device__ __forceinline__ uint64_t l2_evict_first() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ void cp_async16_ef(uint32_t dst, const void* src) {
+    asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "l"(l2_evict_first()) : "memory");
+}
+template <int BYTES>
+__device__ __forceinline__ void cp_async_small_ef(uint32_t dst, const void* src) {
+    asm volatile("cp.async.ca.shared.global.L2::cache_hint [%0], [%1], %2, %3;" ::"r"(dst), "l"(src), "n"(BYTES), "l"(l2_evict_first())
+                 : "memory");
+}
+// read-only global load (the path __ldg takes), evict-first; T: uint8_t, uint16_t, uint32_t or uint4
+template <typename T>
+__device__ __forceinline__ T ldg_ef(const T* p) {
+    const uint64_t pol = l2_evict_first();
+    if constexpr (sizeof(T) == 16) {
+        uint4 v;
+        asm("ld.global.nc.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+            : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(pol));
+        return v;
+    } else if constexpr (sizeof(T) == 4) {
+        uint32_t v;
+        asm("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+        return (T)v;
+    } else if constexpr (sizeof(T) == 2) {
+        unsigned short v;
+        asm("ld.global.nc.L2::cache_hint.u16 %0, [%1], %2;" : "=h"(v) : "l"(p), "l"(pol));
+        return (T)v;
+    } else {
+        static_assert(sizeof(T) == 1, "ldg_ef: 1, 2, 4 or 16 bytes");
+        unsigned short v;
+        asm("ld.global.nc.L2::cache_hint.u8 %0, [%1], %2;" : "=h"(v) : "l"(p), "l"(pol));
+        return (T)v;
+    }
+}
+
 __device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
@@ -183,10 +228,17 @@ __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst_smem, const void* src
                  "l"(src), "r"(bytes), "r"(bar)
                  : "memory");
 }
+// the same, evict-first (l2_evict_first)
+__device__ __forceinline__ void bulk_copy_g2s_ef(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst_smem),
+                 "l"(src), "r"(bytes), "r"(bar), "l"(l2_evict_first())
+                 : "memory");
+}
 
-// bulk prefetch of a global range into L2 (no shared memory, no completion to wait for).  16-byte aligned, size % 16 == 0.
-__device__ __forceinline__ void bulk_prefetch_l2(const void* src, uint32_t bytes) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
+// bulk prefetch of a global range into L2, evict-first (no shared memory, no completion to wait for).  16-byte aligned,
+// size % 16 == 0.
+__device__ __forceinline__ void bulk_prefetch_l2_ef(const void* src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(src), "r"(bytes), "l"(l2_evict_first()) : "memory");
 }
 
 // D(16x8, f32) += A(16x16, f16, row) * B(16x8, f16, col)

@@ -355,6 +355,8 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
     // request stages [s0, s0 + cnt) into their places in the arena: lane j decodes and issues stage s0 + j (cnt <= I8_BARS), so
     // a batch of requests costs one descriptor decode, not one per stage.  `d` is lane j's descriptor (stage s0 + j).  With the
     // stage come its group's scale row (flush stages) and descriptor s + I8_BARS, on the same barrier (see DF_FLUSH above).
+    // Weights and scale rows are read once per step: evict-first in L2.  The descriptor is not: every layer's launch of the same
+    // structure walks the same plan.
     auto issue_stages = [&](int s0, int cnt, uint4 d) {
         if (lane < cnt) {
             const int s = s0 + lane;
@@ -368,8 +370,8 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
             const uint32_t slot = (uint32_t)s & (I8_BARS - 1);
             const uint32_t bar = bar0 + slot * 8u;
             mbar_arrive_expect_tx(bar, bytes + sbytes + (lnext ? 16u : 0u));
-            bulk_copy_g2s(ring + ((d.w >> 16) & 0xffu) * 128u, pk + d.x, bytes, bar);
-            if (sbytes) bulk_copy_g2s(sring + slot * (uint32_t)P.srow, wt + (size_t)d.y * esz, sbytes, bar);
+            bulk_copy_g2s_ef(ring + ((d.w >> 16) & 0xffu) * 128u, pk + d.x, bytes, bar);
+            if (sbytes) bulk_copy_g2s_ef(sring + slot * (uint32_t)P.srow, wt + (size_t)d.y * esz, sbytes, bar);
             if (lnext) bulk_copy_g2s(lwin + ((uint32_t)(s + I8_BARS) & (I8_LWIN - 1)) * 16u, list + s + I8_BARS, 16u, bar);
         }
     };
@@ -394,7 +396,7 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemv_i8_kernel(const __grid_
                 const uint4 d = __ldg(list + s);
                 const uint32_t mi = (d.z >> 22) & 3u;
                 const uint8_t* pk = mi == 0 ? P.mat[0].packed : (mi == 1 ? P.mat[1].packed : P.mat[2].packed);
-                bulk_prefetch_l2(pk + d.x, ((d.z >> 24) & 0xffu) << 7);
+                bulk_prefetch_l2_ef(pk + d.x, ((d.z >> 24) & 0xffu) << 7);
             }
         }
     EXL2B_STAMP(P, 9);
