@@ -299,6 +299,10 @@ def check_branch(sched, kind, calls, dec, L):
             assert len(named(calls, "q_to_fp16_kv")) == len(ref_attn) == len(named(calls, "fp16_to_q_kv"))
         # (prompts of decode schedules run in the decode schedule's flags; their numbers are checked all the same)
         return
+    if kind == "rows_q":        # prefill_rows(cache_attn=True); paged_attn_prefill_q is spied by test_gpu_decoder_prefill_q.PrefillSpy
+        assert len(attn1) == L and len(named(calls, "paged_attn_prefill_q")) == L and len(named(calls, "q_mlp_forward_rows")) == L
+        assert not named(calls, "q_to_fp16_kv") and not named(calls, "fp16_to_q_kv") and not named(calls, "_sdpa_prefill")
+        return
     assert kind == "rows"
     assert len(named(calls, "q_to_fp16_kv")) == L and len(named(calls, "fp16_to_q_kv")) == L
     assert len(attn1) == L and len(named(calls, "q_mlp_forward_rows")) == L
@@ -356,13 +360,21 @@ def row_err(stored, truth, b):
     return np.linalg.norm(s - t, axis=1), np.linalg.norm(rq - t, axis=1), np.linalg.norm(t, axis=1)
 
 
-def check_call(dec, truth, sched, kind, ids, out, pre, post, pos0, chunk=8, floor_ratio=0.0):
+def as_starts(starts, B: int) -> np.ndarray:
+    """Per-sequence first positions of a call: an int array [B], or one int for every sequence."""
+    a = np.asarray(starts, dtype=np.int64).reshape(-1)
+    return np.full(B, int(a[0]), dtype=np.int64) if a.size == 1 else a
+
+
+def check_call(dec, truth, sched, kind, ids, out, pre, post, starts, chunk=8, floor_ratio=0.0, poison=None):
     """What every checked decoder call must satisfy, given the cache snapshots before (pre) and after (post) it and its output
-    (decode: logits [B, vocab]; prompt: hidden state [B, T_last, hidden]):
-      (3) cache_seqlens and dec.pos advanced by exactly the tokens fed, the page table untouched;
+    (decode: logits [B, vocab]; prompt: hidden state [B, T_last, hidden]).  starts: each sequence's position before the call
+    (an int array [B], or one int for all); dec.pos, the host's mirror, must have advanced from max(starts):
+      (3) cache_seqlens advanced by exactly the tokens fed, per sequence, dec.pos with them, the page table untouched;
       (2a) cache bytes at positions written before the call unchanged;
       (2b) each appended row, dequantised, within KV_RATIO x the format's own quantisation error of the truth row (+ slack,
            or FLOOR_RATIO x that row's fp16 floor);
+      (2c) with `poison` (poison_past), every poisoned byte the call did not append into unchanged;
       (1) the output per sequence within OUT_TOL[sched] rel-L2 of the truth, scaled up by floor / FLOOR_TYPICAL where this
           input's fp16 floor is larger than that, and never below floor_ratio x the floor (0: off).
     Returns (worst output rel-L2, worst floor, number of sequences whose bound was scaled)."""
@@ -371,14 +383,19 @@ def check_call(dec, truth, sched, kind, ids, out, pre, post, pos0, chunk=8, floo
     cfg, bits = dec.cfg, dec.cache.wbits
     B, T = ids.shape
     L = cfg.num_layers
+    starts = as_starts(starts, B)
+    assert np.array_equal(pre["seqlens"], starts), (pre["seqlens"], starts)
     assert np.array_equal(post["seqlens"], pre["seqlens"] + T), (pre["seqlens"], post["seqlens"], T)
-    assert dec.pos == pos0 + T
+    assert dec.pos == int(starts.max()) + T
     assert np.array_equal(post["bt"], pre["bt"])
     assert np.isfinite(out).all()
+    if poison is not None:
+        check_poison(poison, post, starts, T)
     kb, vb = kv_q68.widths(bits)
     worst, worst_floor, floored = 0.0, 0.0, 0
     chunks = [(t0, min(chunk, T - t0)) for t0 in range(0, T, chunk)] if kind == "prefill" else [(0, T)]
     for b in range(B):
+        pos0 = int(starts[b])
         pg, r = slots(pre, b, 0, pos0)
         for key in ("k", "ks", "v", "vs"):
             for li in range(L):
@@ -402,8 +419,59 @@ def check_call(dec, truth, sched, kind, ids, out, pre, post, pos0, chunk=8, floo
         bound = max(OUT_TOL[sched] * max(1.0, floor / FLOOR_TYPICAL), floor_ratio * floor)
         floored += bound > OUT_TOL[sched]
         worst, worst_floor = max(worst, err), max(worst_floor, floor)
-        assert err <= bound, f"{sched} seq {b}: rel-L2 {err:.3e} vs the fp64 truth (bound {bound:.3e}, fp16 floor {floor:.3e})"
+        assert err <= bound, (f"{sched} seq {b} (start {pos0}): rel-L2 {err:.3e} vs the fp64 truth (bound {bound:.3e}, "
+                              f"fp16 floor {floor:.3e})")
     return worst, worst_floor, floored
+
+
+# ---- rows past each sequence's length ---------------------------------------------------------------------------------------
+
+# Scales of a poisoned row: codes times scale reach 2^12 before the inverse Hadamard (4-bit codes -8..7 x 2^9, 8-bit codes
+# -128..127 x 2^5), so a dequantised element is at most 2^12 and stays finite in fp16 however the rotation sums it.  Against
+# a live key of norm ~1 such a row scores hundreds to thousands of nats above (or below) every live row: in each head about
+# half of them would take the whole softmax mass if any leaked into a max, a sum or P V.
+POISON_SCALE = {4: 2.0 ** 9, 8: 2.0 ** 5}
+
+
+def poison_rows(rng, shape_q, shape_s, bits):
+    """Random codes at the poison scale: (codes uint8 [shape_q], scales fp16 [shape_s])."""
+    return rng.integers(0, 256, size=shape_q, dtype=np.uint8), np.full(shape_s, POISON_SCALE[bits], dtype=np.float16)
+
+
+def poison_past(dec, lens, rng):
+    """Overwrite every cache row at a position >= lens[b] in sequence b's pages, and every row of a page no sequence owns, in
+    every layer, K and V, with random codes at the poison scale (POISON_SCALE).  Returns the poison: the mask of poisoned
+    (page, row) slots and a snapshot of the cache with it in place, for check_poison."""
+    import kv_q68
+    import torch
+    from exllamav2_b200.model import PAGE_SIZE
+    c = dec.cache
+    kb, vb = kv_q68.widths(c.wbits)
+    bt = c.block_table.cpu().numpy()
+    mask = np.ones((c.key_states[0].shape[0], PAGE_SIZE), dtype=bool)
+    for b, n in enumerate(lens):
+        p = np.arange(int(n))
+        mask[bt[b][p // PAGE_SIZE], p % PAGE_SIZE] = False
+    n = int(mask.sum())
+    idx = tuple(torch.from_numpy(a).to(c.key_states[0].device) for a in np.nonzero(mask))
+    for li in range(dec.cfg.num_layers):
+        for q, s, bits in ((c.key_states[li], c.key_scales[li], kb), (c.value_states[li], c.value_scales[li], vb)):
+            pq, ps = poison_rows(rng, (n,) + tuple(q.shape[2:]), (n,) + tuple(s.shape[2:]), bits)
+            q[idx] = torch.from_numpy(pq).to(q.device)
+            s[idx] = torch.from_numpy(ps).to(s.device)
+    return dict(mask=mask, snap=snapshot(dec))
+
+
+def check_poison(poison, post, starts, T):
+    """Every poisoned slot but the ones this call appended into ([start, start + T) of each sequence) holds the poison's bytes;
+    the appended slots leave the poison."""
+    for b, s in enumerate(starts):
+        pg, r = slots(post, b, int(s), int(s) + T)
+        poison["mask"][pg, r] = False
+    m = poison["mask"]
+    for key in ("k", "ks", "v", "vs"):
+        for li, (a, w) in enumerate(zip(post[key], poison["snap"][key])):
+            assert np.array_equal(a[m].view(np.uint8), w[m].view(np.uint8)), f"layer {li}: a poisoned {key} byte past a length changed"
 
 
 def graph_matches_eager(dec, ids, on_eager=None):
@@ -436,3 +504,84 @@ def graph_matches_eager(dec, ids, on_eager=None):
     assert np.array_equal(eager_cache["seqlens"], replay_cache["seqlens"])
     restore()
     dec.pos -= 1
+
+
+# ---- one un-chained fused decode step (D3 / D6), launch by launch --------------------------------------------------------------
+
+# Per-launch bounds, rel-L2 per sequence against fp64 on the launch's own fp16 inputs: the block entry points' bounds at full
+# size (DESIGN.md §3.7: attention block part 1 / part 2, MLP block, head) and the fused attention's (§3.4).
+LAUNCH_TOL = {"q_attn_forward_1": 1.5e-3, "paged_attn_decode_q4": 1.6e-3, "q_attn_forward_2": 5e-4, "q_mlp_forward_": 3e-3,
+              "rms_norm": 1e-3, "gemm_half_q_half": 5e-4}
+
+
+def replay_fused_step(dec, ids):
+    """One decode step of the fused, un-chained branch (ExLlamaV2Decoder._forward_tokens at q_len 1, then the rms_norm + gemm
+    head), issued here launch by launch on the decoder's own handles and cache, the same calls in the same order.  After each
+    launch its output is compared with fp64 on that launch's own fp16 inputs: weights from get_weight_tensor_dq(), cached rows
+    dequantised by the oracle.  Advances the decoder as decode() would.  Returns {(launch, layer): rel-L2 per sequence [B]}."""
+    import torch
+    import attn_regimes as ar
+    import kv_q68
+    from exllamav2_b200 import ext
+    from exllamav2_b200.model import PAGE_SIZE
+    cfg, c = dec.cfg, dec.cache
+    B, H, KVH, hd, eps = dec.batch_size, cfg.num_heads, cfg.num_kv_heads, cfg.head_dim, cfg.norm_eps
+    kb, vb = kv_q68.widths(c.wbits)
+    f64 = lambda t: t.to(torch.float64)
+    W = [l.get_weight_tensor_dq() for l in dec.linears]
+    out = {}
+
+    def rel(got, want):
+        g, w = f64(got).reshape(B, -1), want.reshape(B, -1)
+        return ((g - w).norm(dim=1) / w.norm(dim=1).clamp_min(1e-30)).cpu().numpy()
+
+    def norm(x, w):
+        x = f64(x)
+        return x / (x * x).mean(-1, keepdim=True).add(eps).sqrt() * f64(w)
+
+    sl = c.cache_seqlens.cpu().numpy().copy()
+    bt = c.block_table.cpu().numpy()
+    pos = torch.as_tensor(sl, device=dec.device)
+    cos, sin = f64(dec.cos)[pos, :hd // 2][:, None, :], f64(dec.sin)[pos, :hd // 2][:, None, :]
+
+    def rope(t, heads):
+        t = t.view(B, heads, hd)
+        l, r = t[..., :hd // 2], t[..., hd // 2:]
+        return torch.cat([l * cos - r * sin, r * cos + l * sin], -1)
+
+    x = dec.embed[torch.as_tensor(ids, device=dec.device).view(-1)].contiguous().view(B, 1, -1)
+    q, k, v = dec.q, dec.k, dec.v
+    ao = dec.attn_out
+    for li, L in enumerate(dec.layers):
+        wq, wk, wv, wo, wg, wu, wd = W[7 * li:7 * li + 7]
+        x0 = x.clone()
+        ext.q_attn_forward_1(L.attn, x, B, 1, -1, c.cache_seqlens, q, k, v, dec.sin, dec.cos)
+        xn = norm(x0.view(B, -1), L.input_norm)
+        want = [rope(xn @ f64(wq), H), rope(xn @ f64(wk), KVH), xn @ f64(wv)]
+        out[("q_attn_forward_1", li)] = np.max([rel(t, w) for t, w in zip((q, k, v), want)], axis=0)
+        # attention: the cached rows [0, seqlen) as the oracle dequantises them, then the unquantised new row
+        qn, kn, vn = (t.view(B, 1, -1, hd).cpu().numpy() for t in (q, k, v))
+        snap = snapshot(dec)
+        Kr = [ar.gather_rows(snap["k"][li], snap["ks"][li], bt, b, int(sl[b]), kb, PAGE_SIZE) for b in range(B)]
+        Vr = [ar.gather_rows(snap["v"][li], snap["vs"][li], bt, b, int(sl[b]), vb, PAGE_SIZE) for b in range(B)]
+        ext.paged_attn_decode_q4(q.view(B, 1, H, hd), k.view(B, 1, KVH, hd), v.view(B, 1, KVH, hd), c.key_states[li],
+                                 c.key_scales[li], c.value_states[li], c.value_scales[li], c.cache_seqlens, c.block_table,
+                                 ao.view(B, 1, H, hd), 1.0 / math.sqrt(hd), wbits=c.wbits)
+        want = torch.as_tensor(ar.attention_truth(qn, kn, vn, Kr, Vr, sl, 1.0 / math.sqrt(hd)), device=dec.device)
+        out[("paged_attn_decode_q4", li)] = rel(ao, want)
+        x0, a0 = x.clone(), ao.clone()
+        ext.q_attn_forward_2(L.attn, x, ao, B, 1)
+        out[("q_attn_forward_2", li)] = rel(x, f64(x0).view(B, -1) + f64(a0).view(B, -1) @ f64(wo))
+        x0 = x.clone()
+        ext.q_mlp_forward_(L.mlp, x)
+        xn = norm(x0.view(B, -1), L.post_norm)
+        g = xn @ f64(wg)
+        out[("q_mlp_forward_", li)] = rel(x, f64(x0).view(B, -1) + (g / (1 + torch.exp(-g)) * (xn @ f64(wu))) @ f64(wd))
+    c.cache_seqlens.add_(1)
+    dec.pos += 1
+    ext.rms_norm(x.view(B, -1), dec.final_norm, dec.xn, eps)
+    out[("rms_norm", -1)] = rel(dec.xn, norm(x.view(B, -1), dec.final_norm))
+    ext.gemm_half_q_half(dec.xn, dec.lm_head.q_handle, dec.logits, False)
+    out[("gemm_half_q_half", -1)] = rel(dec.logits, f64(dec.xn) @ f64(W[-1]))
+    torch.cuda.synchronize()
+    return out

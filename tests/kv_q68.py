@@ -43,6 +43,26 @@ def kv_unpack_q8(packed: np.ndarray, scales: np.ndarray) -> np.ndarray:
     return (v * F16(1.0 / 32.0)).astype(F16)
 
 
+def kv_unpack_exact(packed: np.ndarray, scales: np.ndarray, bits: int) -> np.ndarray:
+    """The stored rows as the fused attention kernels read them: (code - offset) x scale and the inverse Hadamard-32 in fp64,
+    with no rounding.  kv_unpack rounds every step to fp16, as the reference's q_to_fp16_kv does."""
+    p = np.asarray(packed, dtype=np.uint8)
+    if bits == 8:
+        q = p.astype(np.float64) - 128.0
+    else:
+        q = np.empty(p.shape[:-1] + (p.shape[-1] * 2,), dtype=np.float64)
+        q[..., 0::2], q[..., 1::2] = p & 0xF, p >> 4
+        q -= 8.0
+    n = q.shape[-1]
+    w = (q * np.repeat(np.asarray(scales, dtype=np.float64), 32, axis=-1)).reshape(q.shape[:-1] + (n // 64, 32, 2))
+    lane = np.arange(32)
+    i = 1
+    while i < 32:                   # the butterfly of oracle._hadamard32_interleaved, exact
+        w = np.where(((lane & i) != 0)[:, None], -w, w) + w[..., lane ^ i, :]
+        i <<= 1
+    return w.reshape(q.shape) / 32.0
+
+
 def widths(wbits: int) -> tuple[int, int]:
     """Element widths (keys, values) of a cache format."""
     return {4: (4, 4), 6: (8, 4), 8: (8, 8)}[wbits]

@@ -115,8 +115,11 @@ def _truth_model(dec, seed):
     n, hd = dec.sin.shape[0], cfg.head_dim
     ang = np.arange(n)[:, None] * (1.0 / cfg.rope_theta ** (np.arange(0, hd, 2) / hd))[None, :]
     ang = np.concatenate([ang, ang], axis=-1)
+    # (the tables are built in fp32 as the reference builds them: an angle p x f is off by up to ~p x 2^-23 before the fp16
+    # rounding, which matters only for tables much longer than these models' 512 positions)
     for tab, want in ((dec.sin, np.sin(ang)), (dec.cos, np.cos(ang))):
-        assert np.abs(tab.float().cpu().numpy() - want).max() <= 1e-3, "RoPE table differs from sin / cos of position x frequency"
+        assert np.abs(tab.float().cpu().numpy() - want).max() <= 1e-3 + n * 2.0 ** -23, \
+            "RoPE table differs from sin / cos of position x frequency"
 
     def h(t):
         return t.float().cpu().numpy().astype(np.float64)

@@ -113,3 +113,33 @@ def test_q8_pack_layout_and_zero_block():
     assert np.array_equal(kv_q68.kv_unpack_q8(q, s)[0, :64].astype(np.float32), np.zeros(64, dtype=np.float32))
     y = kv_q68.kv_unpack_q8(q, s)[0, 64:].astype(np.float64)
     assert oracle.rel_l2(y, x[0, 64:].astype(np.float64)) < 1e-2
+
+
+def _sylvester(n):
+    h = np.ones((1, 1))
+    while h.shape[0] < n:
+        h = np.block([[h, h], [h, -h]])
+    return h
+
+
+@pytest.mark.parametrize("bits", [4, 8])
+def test_kv_unpack_exact(bits):
+    """kv_q68.kv_unpack_exact: per 64-value unit, each of the two interleaved 32-value halves is H32 (Sylvester order) times
+    (code - offset) x scale, / 32, in fp64 -- restated here with an explicit matrix -- and it agrees with the oracle's fp16
+    dequantisation to that path's roundings."""
+    rng = np.random.default_rng(40 + bits)
+    x = rng.normal(0, 1, size=(64, 2, 128)).astype(np.float16)
+    q, s = kv_q68.kv_pack(x, bits)
+    got = kv_q68.kv_unpack_exact(q, s, bits)
+    if bits == 8:
+        codes = q.astype(np.float64) - 128
+    else:
+        codes = np.empty(q.shape[:-1] + (q.shape[-1] * 2,))
+        codes[..., 0::2], codes[..., 1::2] = q & 0xF, q >> 4
+        codes -= 8
+    w = (codes * np.repeat(s.astype(np.float64), 32, axis=-1)).reshape(codes.shape[:-1] + (-1, 32, 2))
+    want = np.einsum("ij,...jp->...ip", _sylvester(32), w).reshape(codes.shape) / 32
+    assert np.array_equal(got, want)
+    fp16 = kv_q68.kv_unpack(q, s, bits).astype(np.float64)
+    assert np.abs(fp16 - got).max() <= 4e-3 * np.abs(got).max()
+    assert not np.array_equal(fp16, got)
