@@ -9,6 +9,7 @@
 // graph (exllamav2_b200/model.py) streams weights back to back.
 #include "gemv.cuh"
 #include "gemv_i8.cuh"
+#include "lora.cuh"
 
 namespace exl2b {
 
@@ -20,6 +21,7 @@ struct QAttn {
     int device;
     bool i8_qkv;          // q/k/v share K and the row permutation: one gemv_i8 launch for a single row
     half* norm_p;         // the layernorm in q/k/v's stored-row order, taken at creation (single-row launches), or NULL
+    std::vector<LoraAdapter> loras;   // exl2b_qattn_set_loras: projections 0..3 = q, k, v, o
 };
 struct QMlp {
     exl2b_qmlp_desc d;
@@ -27,6 +29,7 @@ struct QMlp {
     bool i8_gu;           // same for gate/up
     half* up_scratch;     // single-row up projection when the caller passes no temp_b (reference: temp_b of make_q_mlp)
     half* norm_p;         // the layernorm in gate/up's stored-row order, as QAttn::norm_p
+    std::vector<LoraAdapter> loras;   // exl2b_qmlp_set_loras: projections 0..2 = gate, up, down
 };
 
 // the handle's copy of its layernorm in the stored-row order of the single-row GEMV's matrices (none without a permutation)
@@ -101,8 +104,10 @@ static bool tc_staged(const QMatrix* const* qs, int n) {
                    "(exl2b_qmatrix_tc_supported)"
 
 // act(norm(x) @ gate) * (norm(x) @ up) -> temp_a as the reference's sequence (q_mlp.cu:78-236): rms_norm, gate and up GEMMs on
-// the dense path (gemm_big.cu), act_mul.  temp_b: rows of scratch for up, or NULL (allocated here)
-static int dense_gate_up(const QMlp* m, const uint16_t* x, int rows, uint16_t* temp_a, uint16_t* temp_b, cudaStream_t stream) {
+// the dense path (gemm_big.cu), act_mul.  temp_b: rows of scratch for up, or NULL (allocated here).  act = false: no act_mul, the
+// raw projections stay in temp_a / temp_b (which must then be given)
+static int dense_gate_up(const QMlp* m, const uint16_t* x, int rows, uint16_t* temp_a, uint16_t* temp_b, cudaStream_t stream,
+                         bool act = true) {
     const exl2b_qmlp_desc& d = m->d;
     const half* xin = (const half*)x;
     half *xn = nullptr, *tb = (half*)temp_b;
@@ -116,9 +121,28 @@ static int dense_gate_up(const QMlp* m, const uint16_t* x, int rows, uint16_t* t
     if (own_tb) EXL2B_CUDA(cudaMallocAsync(&tb, (size_t)rows * d.intermediate_size * sizeof(half), stream));
     int rc = gemm_big_launch((const QMatrix*)d.gate, xin, d.hidden_size, (half*)temp_a, d.intermediate_size, rows, 1, stream);
     if (!rc) rc = gemm_big_launch((const QMatrix*)d.up, xin, d.hidden_size, tb, d.intermediate_size, rows, 1, stream);
-    if (!rc) rc = exl2b_act_mul(temp_a, (const uint16_t*)tb, rows, d.intermediate_size, d.act_gelu, (exl2b_stream_t)stream);
+    if (!rc && act) rc = exl2b_act_mul(temp_a, (const uint16_t*)tb, rows, d.intermediate_size, d.act_gelu, (exl2b_stream_t)stream);
     if (xn) cudaFreeAsync(xn, stream);
     if (own_tb) cudaFreeAsync(tb, stream);
+    return rc;
+}
+
+// rms_norm and the q, k, v GEMMs on the dense path (gemm_big.cu), no rope
+static int dense_qkv(const QAttn* a, const uint16_t* x, int rows, uint16_t* q, uint16_t* k, uint16_t* v, cudaStream_t stream) {
+    const exl2b_qattn_desc& d = a->d;
+    const QMatrix *mq = (const QMatrix*)d.q_proj, *mk = (const QMatrix*)d.k_proj, *mv = (const QMatrix*)d.v_proj;
+    const half* xin = (const half*)x;
+    half* xn = nullptr;
+    if (d.layernorm) {
+        EXL2B_CUDA(cudaMallocAsync(&xn, (size_t)rows * d.hidden_size * sizeof(half), stream));
+        int rc = exl2b_rms_norm(x, d.layernorm, (uint16_t*)xn, d.norm_epsilon, rows, d.hidden_size, (exl2b_stream_t)stream);
+        if (rc) return rc;
+        xin = xn;
+    }
+    int rc = gemm_big_launch(mq, xin, d.hidden_size, (half*)q, mq->v.N, rows, 1, stream);
+    if (!rc) rc = gemm_big_launch(mk, xin, d.hidden_size, (half*)k, mk->v.N, rows, 1, stream);
+    if (!rc) rc = gemm_big_launch(mv, xin, d.hidden_size, (half*)v, mv->v.N, rows, 1, stream);
+    if (xn) cudaFreeAsync(xn, stream);
     return rc;
 }
 
@@ -200,18 +224,7 @@ extern "C" int exl2b_qattn_forward_1_ex(exl2b_qattn_t h, const uint16_t* x, int 
     if ((rows > GEMM_BIG_MIN_ROWS || !tc_staged(qkv, 3)) && !input_prepared && gemm_big_available()) {
         // prefill rows, or groups the wgmma kernel cannot stage: the reference's own sequence (q_attn.cu:153-300) -- rms_norm,
         // three GEMMs, rope -- with the GEMMs on the tensor cores (gemm_big.cu)
-        const half* xin = (const half*)x;
-        half* xn = nullptr;
-        if (d.layernorm) {
-            EXL2B_CUDA(cudaMallocAsync(&xn, (size_t)rows * d.hidden_size * sizeof(half), stream));
-            int rc = exl2b_rms_norm(x, d.layernorm, (uint16_t*)xn, d.norm_epsilon, rows, d.hidden_size, stream_);
-            if (rc) return rc;
-            xin = xn;
-        }
-        int rc = gemm_big_launch(mq, xin, d.hidden_size, (half*)q, mq->v.N, rows, 1, stream);
-        if (!rc) rc = gemm_big_launch(mk, xin, d.hidden_size, (half*)k, mk->v.N, rows, 1, stream);
-        if (!rc) rc = gemm_big_launch(mv, xin, d.hidden_size, (half*)v, mv->v.N, rows, 1, stream);
-        if (xn) cudaFreeAsync(xn, stream);
+        int rc = dense_qkv(a, x, rows, q, k, v, stream);
         if (rc || !rope) return rc;
         const int neox = d.rope_style == 2;
         rc = rope_launch(stream, (half*)q, (const half*)sin, (const half*)cos, batch, q_len * d.num_heads, d.head_dim, d.num_heads,
@@ -483,4 +496,187 @@ extern "C" int exl2b_gemm_half_q_half_norm(exl2b_qmatrix_t h, const uint16_t* x,
         in.x_permuted = 1;
     }
     return gemv_i8_launch(q->device, (cudaStream_t)stream, &o, 1, in);
+}
+
+// ---- LoRA adapters (lora.cu) ------------------------------------------------------------------------------------------------------
+// An adapted stage runs its base GEMMs with the raw outputs stored -- integer GEMV for one row, wgmma for 2..16, the dense path
+// above (or for groups the wgmma kernel cannot stage) -- then one LoRA launch that adds the deltas and finishes the stage.
+// A stage with no active adapter runs exactly as without adapters.
+
+static const int ATTN_STAGES[2][4] = {{0, 1, 2, -1}, {3, -1, -1, -1}};
+static const int MLP_STAGES[2][4] = {{0, 1, -1, -1}, {2, -1, -1, -1}};
+
+extern "C" int exl2b_qattn_set_loras(exl2b_qattn_t h, const exl2b_lora_t* loras, int num, int* max_rank) {
+    QAttn* a = (QAttn*)h;
+    EXL2B_REQUIRE(a, "null argument");
+    const QMatrix* ms[4] = {(const QMatrix*)a->d.q_proj, (const QMatrix*)a->d.k_proj, (const QMatrix*)a->d.v_proj,
+                            (const QMatrix*)a->d.o_proj};
+    int ks[4], ns[4];
+    for (int p = 0; p < 4; ++p) {
+        ks[p] = ms[p] ? ms[p]->v.K : -1;
+        ns[p] = ms[p] ? ms[p]->v.N : -1;
+    }
+    return lora_take(loras, num, ks, ns, 4, ATTN_STAGES, 2, a->loras, max_rank);
+}
+
+extern "C" int exl2b_qmlp_set_loras(exl2b_qmlp_t h, const exl2b_lora_t* loras, int num, int* max_rank) {
+    QMlp* m = (QMlp*)h;
+    EXL2B_REQUIRE(m, "null argument");
+    const QMatrix* ms[3] = {(const QMatrix*)m->d.gate, (const QMatrix*)m->d.up, (const QMatrix*)m->d.down};
+    int ks[3], ns[3];
+    for (int p = 0; p < 3; ++p) {
+        ks[p] = ms[p] ? ms[p]->v.K : -1;
+        ns[p] = ms[p] ? ms[p]->v.N : -1;
+    }
+    return lora_take(loras, num, ks, ns, 3, MLP_STAGES, 2, m->loras, max_rank);
+}
+
+extern "C" int exl2b_qattn_forward_1_lora(exl2b_qattn_t h, const uint16_t* x, int batch, int q_len, int past_len,
+                                          const int32_t* past_lens, uint16_t* q, uint16_t* k, uint16_t* v, const uint16_t* sin,
+                                          const uint16_t* cos, const uint64_t* ids, int num_ids, exl2b_stream_t stream_) {
+    QAttn* a = (QAttn*)h;
+    EXL2B_REQUIRE(a && x && q && k && v && (ids || num_ids == 0), "null argument");
+    LoraParams lp = {};
+    int rc = lora_stack(a->loras, ids, num_ids, ATTN_STAGES[0], 3, lp);
+    if (rc) return rc;
+    if (lp.nseg == 0) return exl2b_qattn_forward_1(h, x, batch, q_len, past_len, past_lens, q, k, v, sin, cos, stream_);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    EXL2B_CUDA(cudaSetDevice(a->device));
+    const exl2b_qattn_desc& d = a->d;
+    const int rows = batch * q_len;
+    const bool rope = d.rope_style != 0 && sin;
+    if (d.rope_style != 0 && rows > 1) EXL2B_REQUIRE(sin && cos, "rope needs sin/cos tables");
+    const QMatrix *mq = (const QMatrix*)d.q_proj, *mk = (const QMatrix*)d.k_proj, *mv = (const QMatrix*)d.v_proj;
+    const QMatrix* qkv[3] = {mq, mk, mv};
+    if (rows == 1 && a->i8_qkv && gemv_i8_enabled()) {
+        const I8Out o[3] = {{mq, (half*)q, 1}, {mk, (half*)k, 1}, {mv, (half*)v, 1}};
+        const I8Input in = {(const half*)x, nullptr, (const half*)d.layernorm, d.norm_epsilon, d.layernorm ? I8_RMSNORM : I8_PLAIN, 0,
+                            a->norm_p};
+        rc = gemv_i8_launch(a->device, stream, o, 3, in);
+    } else if ((rows > GEMM_BIG_MIN_ROWS || !tc_staged(qkv, 3)) && gemm_big_available()) {
+        rc = dense_qkv(a, x, rows, q, k, v, stream);
+    } else {
+        GemvMat mats[3] = {
+            make_mat(mq, (const half*)x, d.hidden_size, (half*)q, mq->v.N, 1),
+            make_mat(mk, (const half*)x, d.hidden_size, (half*)k, mk->v.N, 1),
+            make_mat(mv, (const half*)x, d.hidden_size, (half*)v, mv->v.N, 1),
+        };
+        rc = gemv_launch(a->device, stream, mats, 3, rows, (const half*)d.layernorm, d.norm_epsilon, EPI_STORE);
+    }
+    if (rc) return rc;
+    lp.x = (const half*)x;
+    lp.ldx = lp.K = d.hidden_size;
+    lp.rows = rows;
+    lp.norm_w = (const half*)d.layernorm;
+    lp.norm_eps = d.norm_epsilon;
+    half* ys[3] = {(half*)q, (half*)k, (half*)v};
+    for (int p = 0; p < 3; ++p) {
+        lp.y[p] = ys[p];
+        lp.n[p] = lp.ldy[p] = qkv[p]->v.N;
+    }
+    lp.epi = LORA_QKV;
+    lp.head_dim = d.head_dim;
+    lp.heads_q = d.num_heads;
+    lp.heads_kv = d.num_kv_heads;
+    if (rope) {
+        EXL2B_REQUIRE(d.head_dim % 2 == 0 && d.sincos_size % 4 == 0 && d.sincos_size <= d.head_dim, "rope: bad head_dim/sincos_size");
+        lp.sin = (const half*)sin;
+        lp.cos = (const half*)cos;
+        lp.past_lens = past_lens;
+        lp.past_len = past_len;
+        lp.q_len = q_len;
+        lp.sincos_size = d.sincos_size;
+        lp.neox = d.rope_style == 2;
+    }
+    return lora_launch(a->device, stream, lp);
+}
+
+extern "C" int exl2b_qattn_forward_2_lora(exl2b_qattn_t h, uint16_t* x, const uint16_t* attn_out, int batch, int q_len,
+                                          const uint64_t* ids, int num_ids, exl2b_stream_t stream) {
+    QAttn* a = (QAttn*)h;
+    EXL2B_REQUIRE(a && x && attn_out && (ids || num_ids == 0), "null argument");
+    LoraParams lp = {};
+    int rc = lora_stack(a->loras, ids, num_ids, ATTN_STAGES[1], 1, lp);
+    if (rc) return rc;
+    rc = exl2b_qattn_forward_2(h, x, attn_out, batch, q_len, stream);     // base O (+ residual), un-chained
+    if (rc || lp.nseg == 0) return rc;
+    const QMatrix* mo = (const QMatrix*)a->d.o_proj;
+    lp.x = (const half*)attn_out;
+    lp.ldx = lp.K = mo->v.K;
+    lp.rows = batch * q_len;
+    lp.y[0] = (half*)x;
+    lp.n[0] = lp.ldy[0] = mo->v.N;
+    lp.epi = LORA_ADD;
+    return lora_launch(a->device, (cudaStream_t)stream, lp);
+}
+
+extern "C" int exl2b_qmlp_forward_lora(exl2b_qmlp_t h, uint16_t* x, int rows, uint16_t* temp_a, uint16_t* temp_b,
+                                       const uint64_t* ids, int num_ids, exl2b_stream_t stream_) {
+    QMlp* m = (QMlp*)h;
+    EXL2B_REQUIRE(m && x && temp_a && (ids || num_ids == 0), "null argument");
+    EXL2B_REQUIRE(m->d.down, "this MLP handle was created without down_proj");
+    LoraParams gu = {}, dn = {};
+    int rc = lora_stack(m->loras, ids, num_ids, MLP_STAGES[0], 2, gu);
+    if (!rc) rc = lora_stack(m->loras, ids, num_ids, MLP_STAGES[1], 1, dn);
+    if (rc) return rc;
+    if (gu.nseg == 0 && dn.nseg == 0) return exl2b_qmlp_forward(h, x, rows, temp_a, temp_b, stream_);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    EXL2B_CUDA(cudaSetDevice(m->device));
+    const exl2b_qmlp_desc& d = m->d;
+    const QMatrix *g = (const QMatrix*)d.gate, *u = (const QMatrix*)d.up, *dw = (const QMatrix*)d.down;
+    if (gu.nseg) {
+        // raw gate -> temp_a, raw up -> temp_b; the LoRA launch writes act(gate + delta) * (up + delta) over temp_a
+        half* tb = (half*)temp_b;
+        bool own_tb = false;
+        if (!tb && rows == 1) {
+            if (!m->up_scratch) EXL2B_CUDA(cudaMalloc(&m->up_scratch, (size_t)d.intermediate_size * sizeof(half)));
+            tb = m->up_scratch;
+        } else if (!tb) {
+            EXL2B_CUDA(cudaMallocAsync(&tb, (size_t)rows * d.intermediate_size * sizeof(half), stream));
+            own_tb = true;
+        }
+        const QMatrix* gu2[2] = {g, u};
+        if (rows == 1 && m->i8_gu && gemv_i8_enabled()) {
+            const I8Out o[2] = {{g, (half*)temp_a, 1}, {u, tb, 1}};
+            const I8Input in = {(const half*)x, nullptr, (const half*)d.layernorm, d.norm_epsilon, d.layernorm ? I8_RMSNORM : I8_PLAIN, 0,
+                                m->norm_p};
+            rc = gemv_i8_launch(m->device, stream, o, 2, in);
+        } else if ((rows > GEMM_BIG_MIN_ROWS || !tc_staged(gu2, 2)) && gemm_big_available()) {
+            rc = dense_gate_up(m, x, rows, temp_a, (uint16_t*)tb, stream, false);
+        } else {
+            GemvMat mats[2] = {
+                make_mat(g, (const half*)x, d.hidden_size, (half*)temp_a, d.intermediate_size, 1),
+                make_mat(u, (const half*)x, d.hidden_size, tb, d.intermediate_size, 1),
+            };
+            rc = gemv_launch(m->device, stream, mats, 2, rows, (const half*)d.layernorm, d.norm_epsilon, EPI_STORE);
+        }
+        if (!rc) {
+            gu.x = (const half*)x;
+            gu.ldx = gu.K = d.hidden_size;
+            gu.rows = rows;
+            gu.norm_w = (const half*)d.layernorm;
+            gu.norm_eps = d.norm_epsilon;
+            gu.y[0] = (half*)temp_a;
+            gu.y[1] = tb;
+            gu.n[0] = gu.n[1] = gu.ldy[0] = gu.ldy[1] = d.intermediate_size;
+            gu.epi = LORA_ACT_MUL;
+            gu.act_out = (half*)temp_a;
+            gu.ld_act = d.intermediate_size;
+            gu.gelu = d.act_gelu;
+            rc = lora_launch(m->device, stream, gu);
+        }
+        if (own_tb) cudaFreeAsync(tb, stream);
+    } else {
+        rc = exl2b_qmlp_forward_gateup(h, x, rows, temp_a, stream_);          // temp_a = act(gate) * up
+    }
+    if (rc) return rc;
+    rc = exl2b_gemm_half_q_half(d.down, temp_a, d.intermediate_size, x, d.hidden_size, rows, d.has_residual ? 0 : 1, 0, stream_);
+    if (rc || dn.nseg == 0) return rc;
+    dn.x = (const half*)temp_a;
+    dn.ldx = dn.K = d.intermediate_size;
+    dn.rows = rows;
+    dn.y[0] = (half*)x;
+    dn.n[0] = dn.ldy[0] = dw->v.N;
+    dn.epi = LORA_ADD;
+    return lora_launch(m->device, stream, dn);
 }

@@ -273,6 +273,21 @@ __device__ __forceinline__ void stu128(uint32_t addr, uint4 v) {
 }
 // orders this thread's earlier generic-proxy shared-memory accesses before later async-proxy (bulk copy) writes
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// act(x) of act_mul (cuda/q_mlp_activation.cuh:54-130), shared by act_mul_kernel and the LoRA gate|up epilogue (lora.cu)
+__device__ __forceinline__ half2 silu2(half2 x) {
+    half2 one = __float2half2_rn(1.0f);
+    half2 e = h2exp(__hneg2(x));
+    half2 r = h2rcp(__hadd2(one, e));
+    return __hmul2(x, r);
+}
+__device__ __forceinline__ half gelu1(half x) {
+    float xf = __half2float(x);
+    const float c = 0.797884560803f;
+    float t = c * (xf + 0.044715f * xf * xf * xf), th;
+    asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(t));
+    xf = 0.5f * xf * (1.0 + th);
+    return __float2half_rn(xf);
+}
 #endif
 
 }  // namespace exl2b

@@ -113,20 +113,6 @@ __global__ void rope_kernel(half* __restrict__ x, const half* __restrict__ sin, 
 }
 
 // ---- act * mul: cuda/q_mlp_activation.cuh:54-130 -----------------------------------------------------------------
-__device__ __forceinline__ half2 silu2(half2 x) {
-    half2 one = __float2half2_rn(1.0f);
-    half2 e = h2exp(__hneg2(x));
-    half2 r = h2rcp(__hadd2(one, e));
-    return __hmul2(x, r);
-}
-__device__ __forceinline__ half gelu1(half x) {
-    float xf = __half2float(x);
-    const float c = 0.797884560803f;
-    float t = c * (xf + 0.044715f * xf * xf * xf), th;
-    asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(t));
-    xf = 0.5f * xf * (1.0 + th);
-    return __float2half_rn(xf);
-}
 __global__ void act_mul_kernel(half* __restrict__ x, const half* __restrict__ y, size_t n2, int gelu) {
     griddep_launch_dependents();
     griddep_wait();

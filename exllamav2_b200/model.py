@@ -275,11 +275,68 @@ class ExLlamaV2Decoder:
         # above one row a chained step runs every matrix on the wgmma kernel, which cannot stage groups of 256+ rows (EXL2 or GPTQ
         # g256+, ungrouped GPTQ; include/exl2_b200.h exl2b_qmatrix_tc_supported)
         self.tc_staged = all(ext_c.qmatrix_tc_supported(l.q_handle) for l in self.linears)
+        self.loras: dict[int, list] = {}     # id -> per layer {projection: (A, B)} (load_lora)
+        self.lora_ids: list[int] = []         # the active adapters (set_loras)
+
+    LORA_TARGETS = ("q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj")
+
+    def load_lora(self, rank: int, targets=LORA_TARGETS, scaling: float = 1.0, seed: int = 0) -> int:
+        """Register a synthetic adapter of `rank` on the `targets` projections of every layer and return its id (inactive until
+        set_loras).  A [in, rank] ~ N(0, 1/in) and B [rank, out] ~ N(0, 0.2^2/rank) * scaling: with the decoder's weights (std
+        1/sqrt(in)) the adapter moves each projection's output by about 20 % of its size times `scaling`."""
+        bad = set(targets) - set(self.LORA_TARGETS)
+        if bad:
+            raise ValueError(f"unknown LoRA targets {sorted(bad)}; expected names from {self.LORA_TARGETS}")
+        gen = torch.Generator(device=self.device)
+        gen.manual_seed(seed)
+        layers = []
+        for L in self.layers:
+            mats = dict(zip(self.LORA_TARGETS, (L.q_proj, L.k_proj, L.v_proj, L.o_proj, L.gate, L.up, L.down)))
+            ad = {}
+            for t in self.LORA_TARGETS:
+                if t not in targets:
+                    continue
+                K, N = mats[t].in_features, mats[t].out_features
+                a = (torch.randn((K, rank), device=self.device, generator=gen) / math.sqrt(K)).half()
+                b = (torch.randn((rank, N), device=self.device, generator=gen) * (0.2 * scaling / math.sqrt(rank))).half()
+                ad[t] = (a, b)
+            layers.append(ad)
+        key = id(layers)
+        self.loras[key] = layers
+        self._register_loras()
+        return key
+
+    def unload_lora(self, key: int):
+        """Remove an adapter (and deactivate it)."""
+        del self.loras[key]
+        if key in self.lora_ids:
+            self.set_loras([i for i in self.lora_ids if i != key])
+        self._register_loras()
+
+    def set_loras(self, ids):
+        """Make `ids` (from load_lora) the active adapters of every following step; [] returns to the plain step.  Drops a captured
+        graph: capture() again for the new set."""
+        unknown = [i for i in ids if i not in self.loras]
+        if unknown:
+            raise KeyError(f"no adapter loaded under ids {unknown}")
+        self.lora_ids = list(ids)
+        self.graph = None
+
+    def _register_loras(self):
+        """Every loaded adapter on every block handle (the reference's model.update_loras(), lora.py:194)."""
+        for li, L in enumerate(self.layers):
+            d = {t: ({}, {}) for t in self.LORA_TARGETS}
+            for key, layers in self.loras.items():
+                for t, (a, b) in layers[li].items():
+                    d[t][0][key], d[t][1][key] = a, b
+            ext_c.q_attn_set_loras(L.attn, *d["q_proj"], *d["k_proj"], *d["v_proj"], *d["o_proj"])
+            ext_c.q_mlp_set_loras(L.mlp, *d["gate_proj"], *d["up_proj"], *d["down_proj"])
 
     def _chains(self, rows: int) -> bool:
         """Does a step of `rows` rows (batch x new tokens) run the chained schedule?  One row on the integer GEMV always can;
-        more rows only when every matrix can be staged by the wgmma kernel (otherwise the blocks take the dense path)."""
-        if not (self.chained and self.fused_attn and rows <= 8):
+        more rows only when every matrix can be staged by the wgmma kernel (otherwise the blocks take the dense path).  Never
+        with active adapters: their deltas need each stage's raw outputs in memory (the un-chained block forms)."""
+        if not (self.chained and self.fused_attn and rows <= 8) or self.lora_ids:
             return False
         return self.tc_staged or (rows == 1 and self.row_gemv)
 
@@ -301,16 +358,16 @@ class ExLlamaV2Decoder:
         for li, L in enumerate(self.layers):
             if self.fused_attn and q_len <= 8:
                 # past_len = -1: positions come from cache_seqlens on the device (rope.cu:39-43)
-                ext_c.q_attn_forward_1(L.attn, x, B, q_len, -1, cache.cache_seqlens, q, k, v, self.sin, self.cos)
+                ext_c.q_attn_forward_1(L.attn, x, B, q_len, -1, cache.cache_seqlens, q, k, v, self.sin, self.cos, self.lora_ids)
                 ext_c.paged_attn_decode_q4(q.view(B, q_len, H, hd), k.view(B, q_len, KVH, hd), v.view(B, q_len, KVH, hd),
                                            cache.key_states[li], cache.key_scales[li], cache.value_states[li],
                                            cache.value_scales[li], cache.cache_seqlens, cache.block_table,
                                            attn_out.view(B, q_len, H, hd), 1.0 / math.sqrt(hd), wbits=cache.wbits)
-                ext_c.q_attn_forward_2(L.attn, x, attn_out, B, q_len)
-                ext_c.q_mlp_forward_(L.mlp, x)
+                ext_c.q_attn_forward_2(L.attn, x, attn_out, B, q_len, self.lora_ids)
+                ext_c.q_mlp_forward_(L.mlp, x, self.lora_ids)
                 continue
             tk, tv = cache.get_kv_state(li)
-            ext_c.q_attn_forward_1(L.attn, x, B, q_len, -1, cache.cache_seqlens, q, k, v, self.sin, self.cos)
+            ext_c.q_attn_forward_1(L.attn, x, B, q_len, -1, cache.cache_seqlens, q, k, v, self.sin, self.cos, self.lora_ids)
             rc = _lib.exl2b_paged_attn_decode(q.data_ptr(), k.data_ptr(), v.data_ptr(), tk.data_ptr(), tv.data_ptr(),
                                               cache.cache_seqlens.data_ptr(), cache.block_table.data_ptr(), attn_out.data_ptr(),
                                               B, q_len, cfg.num_heads, cfg.num_kv_heads, cfg.head_dim, PAGE_SIZE,
@@ -318,8 +375,8 @@ class ExLlamaV2Decoder:
             if rc:
                 raise RuntimeError(_lib.exl2b_last_error().decode())
             cache.store_kv_state(li, q_len)
-            ext_c.q_attn_forward_2(L.attn, x, attn_out, B, q_len)
-            ext_c.q_mlp_forward_(L.mlp, x)
+            ext_c.q_attn_forward_2(L.attn, x, attn_out, B, q_len, self.lora_ids)
+            ext_c.q_mlp_forward_(L.mlp, x, self.lora_ids)
         cache.cache_seqlens.add_(q_len)
 
     def _forward_tokens_chained(self, x, q, k, v, attn_out, q_len: int, head: bool = False, gemv_only: bool = False):
@@ -352,7 +409,7 @@ class ExLlamaV2Decoder:
 
     def _decode_step(self):
         torch.index_select(self.embed, 0, self.ids.view(-1), out=self.x.view(self.batch_size, -1))
-        if self.row_gemv and self.batch_size == 1 and self.chained and self.fused_attn:
+        if self.row_gemv and self.batch_size == 1 and self.chained and self.fused_attn and not self.lora_ids:
             self._forward_tokens_chained(self.x, self.q, self.k, self.v, self.attn_out, 1, head=True)
             ext_c.gemv_norm(self.x.view(1, -1), self.lm_head.q_handle, self.final_norm, self.cfg.norm_eps, self.logits, prepared=True)
             return
@@ -440,15 +497,15 @@ class ExLlamaV2Decoder:
         fa = _flash_attn_with_kvcache()
         for li, L in enumerate(self.layers):
             tk, tv = cache.get_kv_state(li)
-            ext_c.q_attn_forward_1(L.attn, x, B, T, -1, cache.cache_seqlens, q, k, v, self.sin, self.cos)
+            ext_c.q_attn_forward_1(L.attn, x, B, T, -1, cache.cache_seqlens, q, k, v, self.sin, self.cos, self.lora_ids)
             if fa is not None:
                 ao = fa(q=q.view(B, T, H, hd), k=k.view(B, T, KVH, hd), v=v.view(B, T, KVH, hd), k_cache=tk, v_cache=tv,
                         cache_seqlens=cache.cache_seqlens, block_table=cache.block_table, causal=True, softmax_scale=1.0 / math.sqrt(hd))
             else:
                 ao = _sdpa_prefill(q.view(B, T, H, hd), k.view(B, T, KVH, hd), v.view(B, T, KVH, hd), tk, tv, cache, hd)
             cache.store_kv_state(li, T)
-            ext_c.q_attn_forward_2(L.attn, x, ao.reshape(B, T, H * hd), B, T)
-            ext_c.q_mlp_forward_rows(L.mlp, x.view(B * T, -1), ta, tb)
+            ext_c.q_attn_forward_2(L.attn, x, ao.reshape(B, T, H * hd), B, T, self.lora_ids)
+            ext_c.q_mlp_forward_rows(L.mlp, x.view(B * T, -1), ta, tb, self.lora_ids)
         cache.cache_seqlens.add_(T)
         return x
 
@@ -467,12 +524,12 @@ class ExLlamaV2Decoder:
         ta = torch.empty((B * T, cfg.intermediate_size), dtype=torch.half, device=self.device)
         tb = torch.empty_like(ta)
         for li, L in enumerate(self.layers):
-            ext_c.q_attn_forward_1(L.attn, x, B, T, -1, cache.cache_seqlens, q, k, v, self.sin, self.cos)
+            ext_c.q_attn_forward_1(L.attn, x, B, T, -1, cache.cache_seqlens, q, k, v, self.sin, self.cos, self.lora_ids)
             ext_c.paged_attn_prefill_q(q.view(B, T, H, hd), k.view(B, T, KVH, hd), v.view(B, T, KVH, hd), cache.key_states[li],
                                        cache.key_scales[li], cache.value_states[li], cache.value_scales[li], cache.cache_seqlens,
                                        cache.block_table, ao.view(B, T, H, hd), 1.0 / math.sqrt(hd), wbits=cache.wbits)
-            ext_c.q_attn_forward_2(L.attn, x, ao, B, T)
-            ext_c.q_mlp_forward_rows(L.mlp, x.view(B * T, -1), ta, tb)
+            ext_c.q_attn_forward_2(L.attn, x, ao, B, T, self.lora_ids)
+            ext_c.q_mlp_forward_rows(L.mlp, x.view(B * T, -1), ta, tb, self.lora_ids)
         cache.cache_seqlens.add_(T)
         return x
 

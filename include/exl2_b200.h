@@ -167,6 +167,50 @@ int exl2b_qmlp_forward(exl2b_qmlp_t h, uint16_t* x, int rows, uint16_t* temp_a, 
  * the residual stream (ldc = hidden size). */
 int exl2b_qmlp_forward_gateup(exl2b_qmlp_t h, const uint16_t* x, int rows, uint16_t* temp_a, exl2b_stream_t stream);
 
+/* ---- LoRA adapters on the blocks ------------------------------------------------------------------------------
+ * q_attn_set_loras / q_mlp_set_loras (ext_qattn.cpp:194-240, ext_qmlp.cpp) and the `loras` argument of q_attn_forward_1 /
+ * q_attn_forward_2 / q_mlp_forward_ (ext_qattn.cpp:115-191, ext_qmlp.cpp:87-118 -> cuda/lora.cu).
+ * For every projection P with an adapter whose id is active: y_P += (in_P · A) · B, A fp16 [in_features, rank] and B fp16
+ * [rank, out_features] (row-major, B already times the adapter's scaling, lora.py:168).  in_P is the RMSNorm'd block input for
+ * q, k, v, gate and up (the delta lands before RoPE / act·mul), attn_output for o and act(gate)·up for down (the delta lands in
+ * the residual stream after the projection has accumulated into it).  All active adapters of a projection are summed in fp32
+ * and y is rounded to fp16 once.
+ * A handle keeps the pointers, not copies: the tensors must outlive the set (the caller's adapter object owns them), and
+ * in-place changes to their contents are seen by the next call, captured graphs included.
+ * Projection index p: attention q 0, k 1, v 2, o 3; MLP gate 0, up 1, down 2. */
+#define EXL2B_LORA_MAX_RANK 512      /* ranks (each rounded up to 8) of all adapters on one stage: q|k|v, o, gate|up or down */
+#define EXL2B_LORA_MAX_ADAPTERS 8    /* adapters one handle holds */
+typedef struct {
+    uint64_t id;                     /* the caller's key (id(lora) in the reference) */
+    const uint16_t* a[4];            /* per projection: A, or NULL for no adapter on it */
+    const uint16_t* b[4];            /* B */
+    int rank[4];
+    int a_rows[4];                   /* in_features of A and out_features of B, checked against the projection's matrix */
+    int b_cols[4];
+} exl2b_lora_t;
+/* Replace the handle's whole set (the reference clear()s, ext_qattn.cpp:208-211); *max_rank = the largest rank in it (the
+ * reference's return value).  Rejects: A without B or B without A, shapes that do not match the matrix, a rank outside 1..512,
+ * more than 8 adapters, an id given twice, and a set whose ranks would sum past EXL2B_LORA_MAX_RANK on any stage if all were
+ * active at once. */
+int exl2b_qattn_set_loras(exl2b_qattn_t h, const exl2b_lora_t* loras, int num, int* max_rank);
+int exl2b_qmlp_set_loras(exl2b_qmlp_t h, const exl2b_lora_t* loras, int num, int* max_rank);
+/* The plain forwards with the call's active adapter ids (ids registered nowhere on the handle are skipped, cuda/lora.cu:20-21).
+ * When no id has an adapter on a stage, that stage runs exactly as exl2b_qattn_forward_1 / _2 / exl2b_qmlp_forward; an adapted
+ * stage runs its base GEMMs with their raw outputs stored, then ONE LoRA launch (csrc/lora.cu) that adds every adapter's delta
+ * and finishes the stage: RoPE of q and k, act(gate)·up, or nothing (o, down). */
+int exl2b_qattn_forward_1_lora(exl2b_qattn_t h, const uint16_t* x, int batch, int q_len, int past_len, const int32_t* past_lens,
+                               uint16_t* q, uint16_t* k, uint16_t* v, const uint16_t* sin, const uint16_t* cos,
+                               const uint64_t* ids, int num_ids, exl2b_stream_t stream);
+int exl2b_qattn_forward_2_lora(exl2b_qattn_t h, uint16_t* x, const uint16_t* attn_out, int batch, int q_len, const uint64_t* ids,
+                               int num_ids, exl2b_stream_t stream);
+int exl2b_qmlp_forward_lora(exl2b_qmlp_t h, uint16_t* x, int rows, uint16_t* temp_a, uint16_t* temp_b, const uint64_t* ids,
+                            int num_ids, exl2b_stream_t stream);
+/* Host only: how one launch stacks the adapters.  ranks [num_adapters][num_projs] (0: none), all adapters active in order;
+ * out per segment: its adapter, projection and first stacked column (each rank takes a multiple of 8 columns); *total = the
+ * stacked width.  Fails, naming the bound, past EXL2B_LORA_MAX_RANK. */
+int exl2b_lora_stack(const int* ranks, int num_adapters, int num_projs, int* seg_adapter, int* seg_proj, int* seg_off, int* num_segs,
+                     int* total);
+
 /* ---- host-buffer entry point (bench.py "e2e"): a fp16[M,K] and c fp16[M,N] are HOST pointers (pinned or
  * pageable); the call copies a to the device, runs gemm_half_q_half, copies c back and waits. */
 int exl2b_gemm_half_q_half_host(exl2b_qmatrix_t h, const uint16_t* a_host, uint16_t* c_host, int m, exl2b_stream_t stream);
