@@ -84,8 +84,8 @@ struct GemvParams {
 // grid.y = ceil(M/4) does, cuda/q_gemm.cu:97).
 int gemv_launch(int device, cudaStream_t stream, GemvMat* mats, int nm, int M, const half* norm_w, float norm_eps,
                 int epilogue, const GemvExtras* ex = nullptr);
-// Many-row path (gemm_big.cu): reconstruct a column window + cuBLAS fp16 GEMM with fp32 accumulation.  Rows above
-// GEMM_BIG_MIN_ROWS take it (below, the packed-row kernels re-read the weights at most twice).
+// Many-row path (gemm_big.cu): reconstruct a column window + cuBLAS fp16 GEMM with fp32 accumulation.  Un-chained launches
+// of more than GEMM_BIG_MIN_ROWS rows take it (below, the packed-row kernels re-read the weights at most twice): row_path.
 constexpr int GEMM_BIG_MIN_ROWS = 16;
 bool gemm_big_available();
 int gemm_big_launch(const QMatrix* q, const half* a, int lda, half* c, int ldc, int M, int clear, cudaStream_t stream);
@@ -94,5 +94,14 @@ int gemm_big_launch(const QMatrix* q, const half* a, int lda, half* c, int ldc, 
 bool gemv_supports_extras(const GemvMat* mats, int nm, int M);
 // can the wgmma kernel stage the matrix's quantisation groups (<= 4 KB per 32-column block)?
 bool gemm_tc_supported(const QMatView& v);
+
+// The kernel that runs one launch over the matrices qs[0..n) for `rows` rows (gemm_half_q_half and every block stage):
+//   ROW_I8     one row, when the matrices can share one integer-GEMV launch (`i8_fusable`: the block handle's cached
+//              gemv_i8_fusable, or LAYOUT_TC for a single matrix) and EXL2B_GEMV does not route rows to the wgmma kernel
+//   ROW_DENSE  more than GEMM_BIG_MIN_ROWS rows, or groups the wgmma kernel cannot stage -- unless the launch is `chained`
+//              (reads or writes another launch's activation buffer, which only the two row kernels do) or cuBLAS is missing
+//   ROW_TC     otherwise: the wgmma kernel through gemv_launch
+enum RowPath : int { ROW_I8, ROW_TC, ROW_DENSE };
+RowPath row_path(int rows, const QMatrix* const* qs, int n, bool i8_fusable, bool chained);
 
 }  // namespace exl2b

@@ -327,14 +327,16 @@ def test_attn_block_every_row_count(fmt, blocks):
 @pytest.mark.parametrize("fmt", list(FORMATS))
 def test_mlp_block_every_row_count(fmt, gelu, blocks):
     """q_mlp_forward_ at every row count, and q_mlp_forward_gateup on a handle made without down (act(gate) * up of a
-    tensor-parallel rank's slice)."""
+    tensor-parallel rank's slice).  Both pick gate|up's kernel by the same rule: wherever q_mlp_forward_ leaves act(gate) * up
+    in temp_a (not fused into the down launch: from 9 rows where the wgmma kernel stages the format, from 2 rows elsewhere),
+    q_mlp_forward_gateup leaves the same bits."""
     from exllamav2_b200 import ext as ext_c
     b = blocks(fmt)
     worst = 0.0
     for rows in ROWS:
         x = b.x(rows)
         act = b.act_truth(x, gelu)
-        h, _ = b.mlp(rows, gelu)
+        h, ta_full = b.mlp(rows, gelu)
         xt = x.clone()
         ext_c.q_mlp_forward_(h, xt)
         err = _rel(xt, x.double() + act @ b.W["d"])
@@ -345,6 +347,8 @@ def test_mlp_block_every_row_count(fmt, gelu, blocks):
         err = _rel(ta, act)
         worst = max(worst, err)
         assert err <= MLP_TOL, f"rows {rows}: gate|up rel_l2 {err:.2e}"
+        if rows >= (9 if FORMATS[fmt][3] else 2):       # below: act(gate) * up goes to down's operand buffer only
+            assert torch.equal(ta, ta_full), f"rows {rows}: gate|up differs from the temp_a of q_mlp_forward_"
         other = b.act_truth(x, not gelu)
         assert _rel(ta, other) > 1e-2, "the other activation fits as well: the test cannot tell them apart"
     print(f"\n{fmt} {'gelu' if gelu else 'silu'}: mlp worst rel-L2 {worst:.2e}")
