@@ -21,6 +21,7 @@
 #include <map>
 #include <mutex>
 
+#include "gemv.cuh"
 #include "gemv_i8.cuh"
 #include "kv_format.cuh"
 #include "qmatrix.cuh"
@@ -55,6 +56,7 @@ struct AttnQ4Params {
     const half* rope_cos;
     int rope_neox, sincos_size;
     int out_plain;          // out_xp is a plain fp16 row (single-row GEMV consumer) instead of the core-matrix operand layout
+    int out_tw;             // token slots of that layout: the consumer launch's wgmma tile (tc_tile of batch * q_len)
     int32_t* err;           // sticky device flag: bit 0 = a sequence ran past its page table (nothing appended, no output)
     // split-KV (long contexts, q_len == 1): grid.z CTAs share one (head, sequence); each attends a contiguous chunk of positions
     // and leaves (max, sum, unnormalised rotated output) in `ws`; the last to arrive (counter) merges.  Chunks are at least
@@ -794,8 +796,8 @@ struct AttnCta {
                 P.out_xp[k0] = __low2half(o2);
                 P.out_xp[k1] = __high2half(o2);
             } else {
-                P.out_xp[(size_t)(k0 >> 3) * 64 + m * 8 + (k0 & 7)] = __low2half(o2);
-                P.out_xp[(size_t)(k1 >> 3) * 64 + m * 8 + (k1 & 7)] = __high2half(o2);
+                P.out_xp[(size_t)(k0 >> 3) * (P.out_tw * 8) + m * 8 + (k0 & 7)] = __low2half(o2);
+                P.out_xp[(size_t)(k1 >> 3) * (P.out_tw * 8) + m * 8 + (k1 & 7)] = __high2half(o2);
             }
         }
     }
@@ -1140,12 +1142,15 @@ extern "C" int exl2b_paged_attn_decode_q(const uint16_t* q, const uint16_t* k_ne
     if (out_consumer) {
         QMatrix* oc = (QMatrix*)out_consumer;
         EXL2B_REQUIRE(oc->v.layout == LAYOUT_TC && oc->v.K == num_heads * head_dim, "out_consumer does not take the attention output");
-        EXL2B_REQUIRE(batch * q_len <= 8, "chained attention output needs at most 8 rows");
-        int rc = qmatrix_chain_buffers(oc);
+        const int rows = batch * q_len;
+        EXL2B_REQUIRE(rows <= GEMV_MAX_CHAIN_ROWS, "chained attention output needs at most %d rows (rows %d)", GEMV_MAX_CHAIN_ROWS, rows);
+        const bool wide = rows > GEMV_MTOK;      // o_proj's launch runs on a wide tile and reads its 64-row buffer
+        int rc = qmatrix_chain_buffers(oc, wide);
         if (rc) return rc;
-        P.out_xp = oc->xp_buf;
+        P.out_xp = wide ? oc->xp_wide : oc->xp_buf;
         P.out_invperm = oc->invperm;
-        P.out_plain = (batch * q_len == 1 && gemv_i8_enabled()) ? 1 : 0;      // the single-row GEMV reads a plain fp16 row
+        P.out_plain = (rows == 1 && gemv_i8_enabled()) ? 1 : 0;      // the single-row GEMV reads a plain fp16 row
+        P.out_tw = tc_tile(rows);
     }
     if (rope_style != 0 && rope_sin && rope_cos) {
         EXL2B_REQUIRE(sincos_size == head_dim, "fused RoPE needs sincos_size == head_dim (partial rotary: apply rope_ first)");

@@ -9,7 +9,8 @@
 //   mlp           norm, gate, up, act, down        5              2  norm + gate|up, then act*mul as down's prologue + residual
 // The chained forms (_ex, exl2b_chain_t) have each launch write the next one's input in that matrix's stored-row order, and
 // every launch carries the programmatic-dependent-launch attribute: the decode step captured in one CUDA graph
-// (exllamav2_b200/model.py) is these 4 launches and attention per layer, streaming weights back to back.
+// (exllamav2_b200/model.py) is these 4 launches and attention per layer, streaming weights back to back.  A chained launch of
+// 9..64 rows runs in one pass on the 32- or 64-row wgmma tile and feeds its consumers' 64-row activation buffers.
 // Which kernel runs a stage (integer GEMV, wgmma, dense) is gemv.cu's row_path.
 #include "gemv.cuh"
 #include "gemv_i8.cuh"
@@ -55,30 +56,36 @@ static GemvMat make_mat(const QMatrix* q, const half* x, int ldx, half* c, int l
     return m;
 }
 
+// A chained launch of `rows` rows reads and writes the 8-row activation buffers (xp_buf / sumsq_buf) up to 8 rows, the 64-row
+// ones (xp_wide / sumsq_wide) above
+static half* chain_xp(const QMatrix* q, int rows) { return rows > GEMV_MTOK ? q->xp_wide : q->xp_buf; }
+static float* chain_sumsq(const QMatrix* q, int rows) { return rows > GEMV_MTOK ? q->sumsq_wide : q->sumsq_buf; }
+
 // epilogue of a producer launch -> the consumers' activation buffers (+ sums of squares when they apply an RMSNorm)
-static int chain_out(GemvExtras& ex, const exl2b_chain_t* next) {
+static int chain_out(GemvExtras& ex, const exl2b_chain_t* next, int rows) {
     if (!next || next->num_consumers <= 0) return 0;
     EXL2B_REQUIRE(next->num_consumers <= GEMV_MAX_MATS, "at most %d chained consumers", GEMV_MAX_MATS);
     for (int i = 0; i < next->num_consumers; ++i) {
         QMatrix* c = (QMatrix*)next->consumers[i];
         EXL2B_REQUIRE(c && c->v.layout == LAYOUT_TC, "chained consumer must be a LAYOUT_TC matrix");
-        int rc = qmatrix_chain_buffers(c);
+        int rc = qmatrix_chain_buffers(c, rows > GEMV_MTOK);
         if (rc) return rc;
-        ex.scat[i] = ScatterTarget{c->xp_buf, c->invperm, (const half*)next->norm_weight};
+        ex.scat[i] = ScatterTarget{chain_xp(c, rows), c->invperm, (const half*)next->norm_weight};
     }
     ex.num_scat = next->num_consumers;
-    if (next->norm_weight) ex.sumsq_out = ((QMatrix*)next->consumers[0])->sumsq_buf;
+    if (next->norm_weight) ex.sumsq_out = chain_sumsq((QMatrix*)next->consumers[0], rows);
     return 0;
 }
 // consumer side: the matrices' inputs were written by a chained producer
-static int chain_in(GemvExtras& ex, GemvMat* mats, const QMatrix* const* qs, int nm, bool has_norm) {
+static int chain_in(GemvExtras& ex, GemvMat* mats, const QMatrix* const* qs, int nm, bool has_norm, int rows) {
     ex.prepared = 1;
     for (int i = 0; i < nm; ++i) {
-        EXL2B_REQUIRE(qs[i]->xp_buf, "input_prepared set, but no chained producer has written this matrix's input");
-        mats[i].xp = qs[i]->xp_buf;
+        EXL2B_REQUIRE(chain_xp(qs[i], rows), "input_prepared set, but no chained producer of %d rows has written this matrix's input",
+                      rows);
+        mats[i].xp = chain_xp(qs[i], rows);
     }
     if (has_norm) {
-        ex.sumsq_in = qs[0]->sumsq_buf;
+        ex.sumsq_in = chain_sumsq(qs[0], rows);
         ex.sumsq_in_strips = (qs[0]->v.K + 127) / 128;
     }
     return 0;
@@ -177,14 +184,14 @@ static int qkv_stage(const QAttn* a, const uint16_t* x, int batch, int q_len, in
     } else {
         GemvMat mats[3];
         for (int i = 0; i < 3; ++i) mats[i] = make_mat(qkv[i], (const half*)x, d.hidden_size, out[i], qkv[i]->v.N, 1);
-        const bool fuse = !raw && gemv_supports_extras(mats, 3, rows) &&
+        const bool fuse = !raw && gemv_supports_extras(mats, 3, rows, chained) &&
                           (!rope || (d.head_dim <= 128 && 128 % d.head_dim == 0 && d.sincos_size <= d.head_dim));
-        EXL2B_REQUIRE(!chained || fuse, CHAIN_RULE, GEMV_MTOK);
+        EXL2B_REQUIRE(!chained || fuse, CHAIN_RULE, GEMV_MAX_CHAIN_ROWS);
         if (fuse) {
             GemvExtras ex = {};
             if (rope) ex.rope = RopeFuse{(const half*)sin, (const half*)cos, past_lens, past_len, q_len, d.head_dim, d.sincos_size, d.rope_style == 2, 3u};
             if (chained) {
-                rc = chain_in(ex, mats, qkv, 3, d.layernorm != nullptr);
+                rc = chain_in(ex, mats, qkv, 3, d.layernorm != nullptr, rows);
                 if (rc) return rc;
             }
             return gemv_launch(a->device, stream, mats, 3, rows, (const half*)d.layernorm, d.norm_epsilon, EPI_STORE, &ex);
@@ -308,12 +315,12 @@ extern "C" int exl2b_qattn_forward_2_ex(exl2b_qattn_t h, uint16_t* x, const uint
         return gemm_big_launch(mo, (const half*)attn_out, mo->v.K, (half*)x, mo->v.N, rows, clear, (cudaStream_t)stream);
     GemvMat m = make_mat(mo, (const half*)attn_out, mo->v.K, (half*)x, mo->v.N, clear);
     if (!chained) return gemv_launch(a->device, (cudaStream_t)stream, &m, 1, rows, nullptr, 0.f, EPI_STORE);
-    EXL2B_REQUIRE(gemv_supports_extras(&m, 1, rows), CHAIN_RULE, GEMV_MTOK);
+    EXL2B_REQUIRE(gemv_supports_extras(&m, 1, rows, true), CHAIN_RULE, GEMV_MAX_CHAIN_ROWS);
     GemvExtras ex = {};
-    int rc = chain_out(ex, next);
+    int rc = chain_out(ex, next, rows);
     if (rc) return rc;
     if (input_prepared) {
-        rc = chain_in(ex, &m, &mo, 1, false);
+        rc = chain_in(ex, &m, &mo, 1, false, rows);
         if (rc) return rc;
     }
     return gemv_launch(a->device, (cudaStream_t)stream, &m, 1, rows, nullptr, 0.f, EPI_STORE, &ex);
@@ -393,8 +400,8 @@ extern "C" int exl2b_qmlp_forward_ex(exl2b_qmlp_t h, uint16_t* x, int rows, uint
         make_mat(u, (const half*)x, d.hidden_size, (half*)temp_a, d.intermediate_size, 1),
     };
     GemvMat down = make_mat(dn, (const half*)temp_a, d.intermediate_size, (half*)x, d.hidden_size, d.has_residual ? 0 : 1);
-    const bool fuse = path == ROW_TC && gemv_supports_extras(gu, 2, rows) && gemv_supports_extras(&down, 1, rows);
-    EXL2B_REQUIRE(fuse || !chained, CHAIN_RULE, GEMV_MTOK);
+    const bool fuse = path == ROW_TC && gemv_supports_extras(gu, 2, rows, chained) && gemv_supports_extras(&down, 1, rows, chained);
+    EXL2B_REQUIRE(fuse || !chained, CHAIN_RULE, GEMV_MAX_CHAIN_ROWS);
     if (!fuse) {
         // act(gate) * up into temp_a, then down (+residual): on the dense path as in q_mlp.cu:78-236, or on the wgmma kernel
         int rc = gate_up_stage(m, path, x, rows, temp_a, (half*)temp_b, true, stream);
@@ -408,20 +415,20 @@ extern "C" int exl2b_qmlp_forward_ex(exl2b_qmlp_t h, uint16_t* x, int rows, uint
     exl2b_chain_t to_down = {};
     to_down.consumers[0] = (exl2b_qmatrix_t)dn;
     to_down.num_consumers = 1;
-    int rc = chain_out(e1, &to_down);
+    int rc = chain_out(e1, &to_down, rows);
     if (rc) return rc;
     if (input_prepared) {
         const QMatrix* qs[2] = {g, u};
-        rc = chain_in(e1, gu, qs, 2, d.layernorm != nullptr);
+        rc = chain_in(e1, gu, qs, 2, d.layernorm != nullptr, rows);
         if (rc) return rc;
     }
     rc = gemv_launch(m->device, stream, gu, 2, rows, (const half*)d.layernorm, d.norm_epsilon,
                      d.act_gelu ? EPI_GELU_MUL : EPI_SILU_MUL, &e1);
     if (rc) return rc;
     GemvExtras e2 = {};
-    rc = chain_out(e2, next);
+    rc = chain_out(e2, next, rows);
     if (rc) return rc;
-    rc = chain_in(e2, &down, &dn, 1, false);
+    rc = chain_in(e2, &down, &dn, 1, false, rows);
     if (rc) return rc;
     return gemv_launch(m->device, stream, &down, 1, rows, nullptr, 0.f, EPI_STORE, &e2);
 }
@@ -449,10 +456,10 @@ extern "C" int exl2b_gemm_half_q_half_prepared(exl2b_qmatrix_t h, uint16_t* c, i
     EXL2B_REQUIRE(ldc >= q->v.N, "leading dimension too small");
     EXL2B_CUDA(cudaSetDevice(q->device));
     GemvMat mt = make_mat(q, nullptr, q->v.K, (half*)c, ldc, clear ? 1 : 0);
-    EXL2B_REQUIRE(gemv_supports_extras(&mt, 1, m), CHAIN_RULE, GEMV_MTOK);
+    EXL2B_REQUIRE(gemv_supports_extras(&mt, 1, m, true), CHAIN_RULE, GEMV_MAX_CHAIN_ROWS);
     GemvExtras ex = {};
     const QMatrix* qc = q;
-    int rc = chain_in(ex, &mt, &qc, 1, has_norm != 0);
+    int rc = chain_in(ex, &mt, &qc, 1, has_norm != 0, m);
     if (rc) return rc;
     return gemv_launch(q->device, (cudaStream_t)stream, &mt, 1, m, nullptr, norm_eps, EPI_STORE, &ex);
 }

@@ -1,6 +1,7 @@
 // Dispatch of gemm_half_q_half over the row count, and the split-K workspace of the wgmma kernel.
 //   1 row        -> gemv_i8.cu   (HBM-bound integer GEMV, the decode path)
-//   2 .. 16 rows -> gemm_tc.cu   (packed weights unpacked into the wgmma A operand in shared memory, 8 rows per pass)
+//   2 .. 16 rows -> gemm_tc.cu   (packed weights unpacked into the wgmma A operand in shared memory, 8 rows per pass; chained
+//                                  launches of up to 64 rows in one pass)
 //   more         -> gemm_big.cu  (reconstruct window + dense tensor-core GEMM: the reference's regime above MAX_Q_GEMM_ROWS)
 // Replaces gemm_half_q_half_cuda (exllamav2_ext/cuda/q_gemm.cu:201-313).
 #include <algorithm>
@@ -21,39 +22,48 @@ unsigned long long* g_dbg_rec = nullptr;      // optional per-CTA records of the
 
 // Split-K workspace, arrival counters and the activation-operand scratch of the wgmma kernel, one set per (device, stream):
 // launches on different streams (or host threads driving different streams) never share scratch.  Created on first use --
-// never inside a stream capture: call once eagerly first, as model.capture() does.
+// never inside a stream capture: call once eagerly first, as model.capture() does.  The wide tiles (chained launches of 9..64
+// rows) get their own workspace and scratch, created on their first launch and never moved: a graph captured before holds the
+// 8-row buffers' addresses.  Both share the counters (a launch touches them only after the previous launch has completed).
 struct TcWorkspace {
     float* ws = nullptr;
     unsigned int* counters = nullptr;
     half* xp = nullptr;
     size_t ws_bytes = 0, xp_bytes = 0;
     int n_counters = 0;
+    float* ws_wide = nullptr;
+    half* xp_wide = nullptr;
 };
 static std::map<std::pair<int, cudaStream_t>, TcWorkspace> g_tc_ws;
 static std::mutex g_ws_mutex;
 
-int gemv_workspace(int device, cudaStream_t stream, float** ws, unsigned int** counters, size_t* ws_bytes, int* n_counters, half** xp,
-                   size_t xp_bytes) {
+int gemv_workspace(int device, cudaStream_t stream, bool wide, float** ws, unsigned int** counters, size_t* ws_bytes, int* n_counters,
+                   half** xp, size_t* xp_bytes) {
     std::lock_guard<std::mutex> lock(g_ws_mutex);
     TcWorkspace& d = g_tc_ws[{device, stream}];
     if (!d.ws) {
-        d.ws_bytes = (size_t)32 << 20;
+        d.ws_bytes = TC_WS_BYTES;
         d.n_counters = 1 << 16;
         EXL2B_CUDA(cudaMalloc(&d.ws, d.ws_bytes));
         EXL2B_CUDA(cudaMalloc(&d.counters, d.n_counters * sizeof(unsigned int)));
         EXL2B_CUDA(cudaMemset(d.counters, 0, d.n_counters * sizeof(unsigned int)));
         EXL2B_CUDA(cudaDeviceSynchronize());
     }
-    if (d.xp_bytes < xp_bytes) {
-        if (d.xp) EXL2B_CUDA(cudaFree(d.xp));
-        EXL2B_CUDA(cudaMalloc(&d.xp, xp_bytes));
-        d.xp_bytes = xp_bytes;
+    if (!d.xp) {
+        EXL2B_CUDA(cudaMalloc(&d.xp, TC_XP_BYTES));
+        d.xp_bytes = TC_XP_BYTES;
     }
-    *ws = d.ws;
+    if (wide && !d.ws_wide) {
+        EXL2B_CUDA(cudaMalloc(&d.ws_wide, TC_WIDE_WS_BYTES));
+        EXL2B_CUDA(cudaMalloc(&d.xp_wide, TC_WIDE_XP_BYTES));
+        EXL2B_CUDA(cudaDeviceSynchronize());
+    }
+    *ws = wide ? d.ws_wide : d.ws;
     *counters = d.counters;
-    *ws_bytes = d.ws_bytes;
+    *ws_bytes = wide ? TC_WIDE_WS_BYTES : d.ws_bytes;
     *n_counters = d.n_counters;
-    *xp = d.xp;
+    *xp = wide ? d.xp_wide : d.xp;
+    *xp_bytes = wide ? TC_WIDE_XP_BYTES : d.xp_bytes;
     return 0;
 }
 
@@ -61,10 +71,10 @@ int gemm_tc_launch(int device, cudaStream_t stream, GemvMat* mats, int nm, int M
                    const GemvExtras* ex);
 
 bool gemm_tc_supported(const QMatView& v);
-bool gemv_supports_extras(const GemvMat* mats, int nm, int M) {
+bool gemv_supports_extras(const GemvMat* mats, int nm, int M, bool chained) {
     for (int i = 0; i < nm; ++i)
         if (mats[i].w.layout != LAYOUT_TC || !gemm_tc_supported(mats[i].w)) return false;
-    return M >= 1 && M <= GEMV_MTOK;
+    return M >= 1 && M <= (chained ? GEMV_MAX_CHAIN_ROWS : GEMV_MTOK);
 }
 
 int gemv_launch(int device, cudaStream_t stream, GemvMat* mats, int nm, int M, const half* norm_w, float norm_eps,
@@ -173,7 +183,7 @@ int attn_scratch_query(int device, cudaStream_t stream, int kind, void** ptr, si
 }
 extern "C" int exl2b_debug_scratch(int device, exl2b_stream_t stream, int kind, void** ptr, size_t* bytes) {
     EXL2B_REQUIRE(ptr && bytes && device >= 0 && device < 64, "bad argument");
-    EXL2B_REQUIRE(kind >= EXL2B_SCRATCH_ATTN_WS && kind <= EXL2B_SCRATCH_TC_XP, "unknown scratch kind %d", kind);
+    EXL2B_REQUIRE(kind >= EXL2B_SCRATCH_ATTN_WS && kind <= EXL2B_SCRATCH_TC_XP_WIDE, "unknown scratch kind %d", kind);
     if (kind == EXL2B_SCRATCH_ATTN_WS || kind == EXL2B_SCRATCH_ATTN_CNT)
         return attn_scratch_query(device, (cudaStream_t)stream, kind, ptr, bytes);
     std::lock_guard<std::mutex> lock(g_ws_mutex);
@@ -185,5 +195,7 @@ extern "C" int exl2b_debug_scratch(int device, exl2b_stream_t stream, int kind, 
     if (kind == EXL2B_SCRATCH_TC_WS) { *ptr = d.ws; *bytes = d.ws_bytes; }
     if (kind == EXL2B_SCRATCH_TC_CNT) { *ptr = d.counters; *bytes = (size_t)d.n_counters * sizeof(unsigned int); }
     if (kind == EXL2B_SCRATCH_TC_XP) { *ptr = d.xp; *bytes = d.xp_bytes; }
+    if (kind == EXL2B_SCRATCH_TC_WS_WIDE && d.ws_wide) { *ptr = d.ws_wide; *bytes = TC_WIDE_WS_BYTES; }
+    if (kind == EXL2B_SCRATCH_TC_XP_WIDE && d.xp_wide) { *ptr = d.xp_wide; *bytes = TC_WIDE_XP_BYTES; }
     return 0;
 }

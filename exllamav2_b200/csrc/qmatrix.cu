@@ -470,14 +470,17 @@ extern "C" int exl2b_qmatrix_create(const exl2b_qmatrix_desc* d, exl2b_stream_t 
 }
 
 namespace exl2b {
-int qmatrix_chain_buffers(QMatrix* m) {
-    if (m->xp_buf) return 0;
+int qmatrix_chain_buffers(QMatrix* m, bool wide) {
+    half*& xp = wide ? m->xp_wide : m->xp_buf;
+    float*& sq = wide ? m->sumsq_wide : m->sumsq_buf;
+    if (xp) return 0;
     EXL2B_CUDA(cudaSetDevice(m->device));
-    const size_t xp_bytes = (size_t)m->v.K * 16, sq_bytes = ((size_t)m->v.K / 128 + 2) * 8 * sizeof(float);
-    EXL2B_CUDA(cudaMalloc(&m->xp_buf, xp_bytes));
-    EXL2B_CUDA(cudaMalloc(&m->sumsq_buf, sq_bytes));
-    EXL2B_CUDA(cudaMemset(m->xp_buf, 0, xp_bytes));
-    EXL2B_CUDA(cudaMemset(m->sumsq_buf, 0, sq_bytes));
+    const size_t slots = wide ? 64 : 8;      // token slots of the layout: the widest tile of the row range
+    const size_t xp_bytes = (size_t)m->v.K * 2 * slots, sq_bytes = ((size_t)m->v.K / 128 + 2) * slots * sizeof(float);
+    EXL2B_CUDA(cudaMalloc(&xp, xp_bytes));
+    EXL2B_CUDA(cudaMalloc(&sq, sq_bytes));
+    EXL2B_CUDA(cudaMemset(xp, 0, xp_bytes));
+    EXL2B_CUDA(cudaMemset(sq, 0, sq_bytes));
     return 0;
 }
 }  // namespace exl2b
@@ -491,6 +494,8 @@ extern "C" int exl2b_qmatrix_destroy(exl2b_qmatrix_t h) {
     if (m->wtab) cudaFree(m->wtab);
     if (m->xp_buf) cudaFree(m->xp_buf);
     if (m->sumsq_buf) cudaFree(m->sumsq_buf);
+    if (m->xp_wide) cudaFree(m->xp_wide);
+    if (m->sumsq_wide) cudaFree(m->sumsq_wide);
     delete m;
     return 0;
 }

@@ -49,10 +49,14 @@ struct QMatrix {
     void* wtab = nullptr;               // dense per-(group, column) scale table of the batch-1 GEMV (gemv_i8.cu): EXL2 fp16[G][N] =
                                         //   dq_scale(q_scale nibble, q_scale_max); GPTQ uint32[G][N] = fp16 scale | (qzero + 1) << 16
     half* xp_buf = nullptr;             // chained launches: this matrix's input, written by its producer's epilogue
-    float* sumsq_buf = nullptr;         //   and the producer's per-strip sums of squares (deferred RMSNorm)
+    float* sumsq_buf = nullptr;         //   and the producer's per-strip sums of squares (deferred RMSNorm); 1..8 rows: K x 16 B
+                                        //   (8 token slots), [strips][8]
+    half* xp_wide = nullptr;            // the same for chained launches of 9..64 rows: K x 128 B (64 token slots), [strips][64]
+    float* sumsq_wide = nullptr;
 };
-// allocate xp_buf / sumsq_buf on first use (never inside a stream capture: call once eagerly first)
-int qmatrix_chain_buffers(QMatrix* m);
+// allocate xp_buf / sumsq_buf (wide: xp_wide / sumsq_wide) on first use (never inside a stream capture: call once eagerly
+// first).  Neither pair is ever moved or regrown: a graph captured over one stays valid when the other is created.
+int qmatrix_chain_buffers(QMatrix* m, bool wide = false);
 
 inline uint32_t meta_group(uint32_t m) { return m & 0xFFFFu; }
 inline uint32_t meta_bits(uint32_t m) { return (m >> 16) & 0xFu; }

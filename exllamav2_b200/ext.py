@@ -739,7 +739,7 @@ def paged_attn_status(device) -> int:
 
 
 # include/exl2_b200.h EXL2B_SCRATCH_*
-SCRATCH_KINDS = {"attn_ws": 0, "attn_cnt": 1, "tc_ws": 2, "tc_cnt": 3, "tc_xp": 4}
+SCRATCH_KINDS = {"attn_ws": 0, "attn_cnt": 1, "tc_ws": 2, "tc_cnt": 3, "tc_xp": 4, "tc_ws_wide": 5, "tc_xp_wide": 6}
 
 
 def debug_scratch(device, stream, kind: str) -> tuple[int, int]:

@@ -30,6 +30,10 @@ _lib.exl2b_paged_attn_decode.restype = ctypes.c_int
 _lib.exl2b_paged_attn_decode.argtypes = [ctypes.c_void_p] * 8 + [ctypes.c_int] * 7 + [ctypes.c_float, ctypes.c_void_p]
 
 PAGE_SIZE = 256       # exllamav2/generator/dynamic.py: page = 256 tokens
+# rows of one step (csrc/gemv.cuh): above GEMM_BIG_MIN_ROWS an un-chained stage takes the dense path; a decode step of up to
+# DECODE_CHAIN_ROWS sequences runs chained on the 32-row wgmma tile instead (_chains)
+GEMM_BIG_MIN_ROWS = 16
+DECODE_CHAIN_ROWS = 32
 
 
 @dataclass
@@ -332,11 +336,15 @@ class ExLlamaV2Decoder:
             ext_c.q_attn_set_loras(L.attn, *d["q_proj"], *d["k_proj"], *d["v_proj"], *d["o_proj"])
             ext_c.q_mlp_set_loras(L.mlp, *d["gate_proj"], *d["up_proj"], *d["down_proj"])
 
-    def _chains(self, rows: int) -> bool:
+    def _chains(self, rows: int, q_len: int = 1) -> bool:
         """Does a step of `rows` rows (batch x new tokens) run the chained schedule?  One row on the integer GEMV always can;
-        more rows only when every matrix can be staged by the wgmma kernel (otherwise the blocks take the dense path).  Never
-        with active adapters: their deltas need each stage's raw outputs in memory (the un-chained block forms)."""
-        if not (self.chained and self.fused_attn and rows <= 8) or self.lora_ids:
+        more rows only when every matrix can be staged by the wgmma kernel (otherwise the blocks take the dense path): up to 8
+        rows in any step, and a decode step (one new token per sequence) of 17..32 sequences on the 32-row wgmma tile, which
+        reads the packed weights once where the un-chained step reconstructs every matrix.  Above 32 sequences the 64-row tile
+        measured slower than the dense path on the 7B preset (DESIGN.md §7), so those steps stay un-chained.  Never with active
+        adapters: their deltas need each stage's raw outputs in memory (the un-chained block forms)."""
+        wide = q_len == 1 and GEMM_BIG_MIN_ROWS < rows <= DECODE_CHAIN_ROWS
+        if not (self.chained and self.fused_attn and (rows <= 8 or wide)) or self.lora_ids:
             return False
         return self.tc_staged or (rows == 1 and self.row_gemv)
 
@@ -353,7 +361,7 @@ class ExLlamaV2Decoder:
         B = self.batch_size
         stream = torch.cuda.current_stream(self.device).cuda_stream
         H, KVH, hd = cfg.num_heads, cfg.num_kv_heads, cfg.head_dim
-        if self._chains(B * q_len):
+        if self._chains(B * q_len, q_len):
             return self._forward_tokens_chained(x, q, k, v, attn_out, q_len)
         for li, L in enumerate(self.layers):
             if self.fused_attn and q_len <= 8:

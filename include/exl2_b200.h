@@ -68,7 +68,7 @@ typedef struct exl2b_qmatrix_desc {
 int exl2b_qmatrix_create(const exl2b_qmatrix_desc* desc, exl2b_stream_t stream, exl2b_qmatrix_t* out);
 int exl2b_qmatrix_destroy(exl2b_qmatrix_t h);                     /* free_q_matrix, ext_qmatrix.cpp:187-194 */
 int exl2b_qmatrix_info(exl2b_qmatrix_t h, int* height, int* width, int* groups, int* is_gptq, uint64_t* packed_bytes);
-/* *supported = 1 if the 2..16-row kernel (and with it every chained launch above one row) can run this matrix: it stages one
+/* *supported = 1 if the wgmma kernel (2..16 rows, and every chained launch of 2..64 rows) can run this matrix: it stages one
  * quantisation group of a 32-column block at a time, at most 128 rows (4 KB at 8 bits).  Matrices with larger groups (EXL2 or
  * GPTQ g256+, ungrouped GPTQ) take the dense path at every row count above one instead, and cannot be chained there. */
 int exl2b_qmatrix_tc_supported(exl2b_qmatrix_t h, int* supported);
@@ -243,6 +243,8 @@ enum {
     EXL2B_SCRATCH_TC_WS = 2,     /* split-K workspace of the wgmma kernel */
     EXL2B_SCRATCH_TC_CNT = 3,    /* its arrival counters */
     EXL2B_SCRATCH_TC_XP = 4,     /* its activation-operand scratch */
+    EXL2B_SCRATCH_TC_WS_WIDE = 5,   /* split-K workspace of the 32- and 64-row tiles (chained launches of 9..64 rows) */
+    EXL2B_SCRATCH_TC_XP_WIDE = 6,   /* their activation-operand scratch; both created on the first such launch, never moved */
 };
 int exl2b_debug_scratch(int device, exl2b_stream_t stream, int kind, void** ptr, size_t* bytes);
 
@@ -267,7 +269,7 @@ int exl2b_paged_attn_decode(const uint16_t* q, const uint16_t* k_new, const uint
  * none).  Needs sincos_size == head_dim.
  * `out_consumer` (or NULL): the matrix that takes the attention output (o_proj); the output is also left in its activation
  * buffer (chained launches, below) -- as a plain fp16 row in its stored-row order when there is a single row, where the
- * batch-1 GEMV reads it.
+ * batch-1 GEMV reads it, and in the operand layout of the launch's token tile otherwise.  At most 64 rows (batch * q_len).
  * Cache length: with q_len 2..8 every CTA holds one fp32 score per position of its share of the cache's capacity
  * (pages_per_seq * page_size) in shared memory, so capacities above ~29 000 positions (hd 128) are refused ("context of N
  * tokens does not fit the score buffer").  A single-token step (q_len 1) whose scores do not fit walks each CTA's positions
@@ -305,7 +307,10 @@ int exl2b_paged_attn_clear_status(int device);
  * activation buffer of the matrices that consume it -- permuted through their q_invperm, in the tensor-core operand
  * layout, pre-multiplied by the RMSNorm weight they apply -- together with per-strip sums of squares; the consumer
  * launch (`input_prepared` = 1) then starts without a prep kernel and applies 1/rms to its fp32 result.
- * Valid for rows <= 8 (decode) and the default (LAYOUT_TC) matrix layout; the calls fail otherwise.
+ * Valid for rows <= 64 and the default (LAYOUT_TC) matrix layout with groups the wgmma kernel can stage
+ * (exl2b_qmatrix_tc_supported); the calls fail otherwise.  Each launch runs its rows in one pass on the narrowest token tile
+ * that holds them -- 8 (1..8 rows), 32 (9..32) or 64 (33..64) -- and a producer and its consumers must run the same row
+ * count: 1..8 rows use the matrix's 8-row activation buffer, 9..64 rows a separate 64-row one. 
  * `out_consumer` of exl2b_paged_attn_decode_q is the same mechanism for the attention output (o_proj). */
 typedef struct {
     exl2b_qmatrix_t consumers[3];   /* matrices whose INPUT is this launch's output (e.g. the next block's q, k, v) */
