@@ -240,6 +240,83 @@ static int gate_up_stage(QMlp* m, RowPath path, const uint16_t* x, int rows, uin
                        !act ? EPI_STORE : d.act_gelu ? EPI_GELU_MUL : EPI_SILU_MUL);
 }
 
+// Mirror p of a one-row LoRA launch: the copy of that output a chained producer leaves in `next`'s first consumer (chain_out_i8)
+static int lora_mirror(LoraParams& lp, int p, const exl2b_chain_t* next, int slot = 0) {
+    I8Out o = {};
+    int rc = chain_out_i8(o, next, slot);
+    lp.mirror[p] = o.c_perm;
+    lp.mirror_invperm[p] = o.out_invperm;
+    return rc;
+}
+
+// Adapters on a chained call: the LoRA launch adds its deltas after the producer, which needs the single-row integer GEMV
+static int lora_chain_rule(int rows, RowPath path) {
+    EXL2B_REQUIRE(rows == 1,
+                  "LoRA adapters on a chained call of %d rows: above one row the chained launches fuse RoPE, act(gate)*up and the "
+                  "RMSNorm sums of squares into their epilogues, so no delta can be added after them (use the un-chained forms)",
+                  rows);
+    EXL2B_REQUIRE(path == ROW_I8, "LoRA adapters on a chained call need the single-row integer GEMV (not EXL2B_GEMV=tc)");
+    return 0;
+}
+
+// The single-row MLP on the integer GEMV: gate|up in one launch with RMSNorm as its prologue; act(gate) * up is the PROLOGUE of
+// the down launch, which reads both rows in its own stored-row order (scattered there by the gate|up launch's finalisation).
+// gu / dn (or NULL): the stages' LoRA launches, each after its base launch, in the one-row form: gate|up's adds its deltas to
+// both rows and to down's copies of them, down's forms act(gate)·up from the plain rows and adds to x and to next's copy.
+static int mlp_row(QMlp* m, uint16_t* x, uint16_t* temp_a, uint16_t* temp_b, int input_prepared, const exl2b_chain_t* next,
+                   LoraParams* gu, LoraParams* dn, cudaStream_t stream) {
+    const exl2b_qmlp_desc& d = m->d;
+    const QMatrix *g = (const QMatrix*)d.gate, *u = (const QMatrix*)d.up, *dm = (const QMatrix*)d.down;
+    half* tb = (half*)temp_b;
+    int rc = tb ? 0 : up_row(m, &tb);
+    if (!rc) rc = qmatrix_chain_buffers(const_cast<QMatrix*>(dm));
+    if (rc) return rc;
+    I8Out o[2] = {{g, (half*)temp_a, 1}, {u, tb, 1}};
+    o[0].c_perm = dm->xp_buf;
+    o[1].c_perm = dm->xp_buf + dm->v.K;
+    o[0].out_invperm = o[1].out_invperm = dm->invperm;
+    I8Input in1;
+    rc = i8_input(in1, x, input_prepared, g, "gate_proj", d.layernorm, d.norm_epsilon, m->norm_p);
+    if (!rc) rc = gemv_i8_launch(m->device, stream, o, 2, in1);
+    if (rc) return rc;
+    if (gu && gu->nseg) {
+        gu->x = (const half*)x;
+        gu->ldx = gu->K = d.hidden_size;
+        gu->rows = 1;
+        gu->norm_w = (const half*)d.layernorm;
+        gu->norm_eps = d.norm_epsilon;
+        gu->y[0] = (half*)temp_a;
+        gu->y[1] = tb;
+        gu->n[0] = gu->n[1] = gu->ldy[0] = gu->ldy[1] = d.intermediate_size;
+        gu->epi = LORA_ADD_PAIR;
+        gu->one_row = 1;
+        for (int p = 0; p < 2; ++p) {
+            gu->mirror[p] = o[p].c_perm;
+            gu->mirror_invperm[p] = o[p].out_invperm;
+        }
+        rc = lora_launch(m->device, stream, *gu);
+        if (rc) return rc;
+    }
+    I8Out od = {dm, (half*)x, d.has_residual ? 0 : 1};
+    rc = chain_out_i8(od, next);
+    if (rc) return rc;
+    const I8Input in2 = {dm->xp_buf, dm->xp_buf + dm->v.K, nullptr, 0.f, d.act_gelu ? I8_GELU_MUL : I8_SILU_MUL, 1};
+    rc = gemv_i8_launch(m->device, stream, &od, 1, in2);
+    if (rc || !dn || !dn->nseg) return rc;
+    dn->x = (const half*)temp_a;
+    dn->x2 = tb;
+    dn->gelu = d.act_gelu;
+    dn->ldx = dn->K = d.intermediate_size;
+    dn->rows = 1;
+    dn->y[0] = (half*)x;
+    dn->n[0] = dn->ldy[0] = d.hidden_size;
+    dn->epi = LORA_ADD;
+    dn->one_row = 1;
+    dn->mirror[0] = od.c_perm;
+    dn->mirror_invperm[0] = od.out_invperm;
+    return lora_launch(m->device, stream, *dn);
+}
+
 }  // namespace exl2b
 
 using namespace exl2b;
@@ -374,27 +451,7 @@ extern "C" int exl2b_qmlp_forward_ex(exl2b_qmlp_t h, uint16_t* x, int rows, uint
     const QMatrix* gud[3] = {g, u, dn};
     const bool chained = input_prepared || (next && next->num_consumers > 0);
     const RowPath path = row_path(rows, gud, 3, m->i8_gu && dn->v.layout == LAYOUT_TC, chained);
-    if (path == ROW_I8) {
-        // decode row: gate|up in one launch with RMSNorm as its prologue; act(gate) * up is the PROLOGUE of the down launch,
-        // which reads both rows in its own stored-row order (scattered there by the gate|up launch's finalisation)
-        half* tb = (half*)temp_b;
-        int rc = tb ? 0 : up_row(m, &tb);
-        if (!rc) rc = qmatrix_chain_buffers(const_cast<QMatrix*>(dn));
-        if (rc) return rc;
-        I8Out o[2] = {{g, (half*)temp_a, 1}, {u, tb, 1}};
-        o[0].c_perm = dn->xp_buf;
-        o[1].c_perm = dn->xp_buf + dn->v.K;
-        o[0].out_invperm = o[1].out_invperm = dn->invperm;
-        I8Input in1;
-        rc = i8_input(in1, x, input_prepared, g, "gate_proj", d.layernorm, d.norm_epsilon, m->norm_p);
-        if (!rc) rc = gemv_i8_launch(m->device, stream, o, 2, in1);
-        if (rc) return rc;
-        I8Out od = {dn, (half*)x, d.has_residual ? 0 : 1};
-        rc = chain_out_i8(od, next);
-        if (rc) return rc;
-        const I8Input in2 = {dn->xp_buf, dn->xp_buf + dn->v.K, nullptr, 0.f, d.act_gelu ? I8_GELU_MUL : I8_SILU_MUL, 1};
-        return gemv_i8_launch(m->device, stream, &od, 1, in2);
-    }
+    if (path == ROW_I8) return mlp_row(m, x, temp_a, temp_b, input_prepared, next, nullptr, nullptr, stream);
     GemvMat gu[2] = {
         make_mat(g, (const half*)x, d.hidden_size, (half*)temp_a, d.intermediate_size, 1),
         make_mat(u, (const half*)x, d.hidden_size, (half*)temp_a, d.intermediate_size, 1),
@@ -527,23 +584,20 @@ extern "C" int exl2b_qmlp_set_loras(exl2b_qmlp_t h, const exl2b_lora_t* loras, i
     return lora_take(loras, num, ks, ns, 3, MLP_STAGES, 2, m->loras, max_rank);
 }
 
-extern "C" int exl2b_qattn_forward_1_lora(exl2b_qattn_t h, const uint16_t* x, int batch, int q_len, int past_len,
-                                          const int32_t* past_lens, uint16_t* q, uint16_t* k, uint16_t* v, const uint16_t* sin,
-                                          const uint16_t* cos, const uint64_t* ids, int num_ids, exl2b_stream_t stream_) {
-    QAttn* a = (QAttn*)h;
-    EXL2B_REQUIRE(a && x && q && k && v && (ids || num_ids == 0), "null argument");
-    LoraParams lp = {};
-    int rc = lora_stack(a->loras, ids, num_ids, ATTN_STAGES[0], 3, lp);
-    if (rc) return rc;
-    if (lp.nseg == 0) return exl2b_qattn_forward_1(h, x, batch, q_len, past_len, past_lens, q, k, v, sin, cos, stream_);
-    cudaStream_t stream = (cudaStream_t)stream_;
+// The adapted q|k|v stage (lp: its stacked adapters): the raw projections, then the LoRA launch that adds the deltas and applies
+// RoPE.  chained: the base launch reads the row a producer left in q's activation buffer (one row); x, the same row in feature
+// order, is the LoRA launch's input.  Without RoPE there the launch takes the one-row form and attention rotates q and k.
+static int qkv_lora(QAttn* a, LoraParams& lp, const uint16_t* x, int batch, int q_len, int past_len, const int32_t* past_lens,
+                    uint16_t* q, uint16_t* k, uint16_t* v, const uint16_t* sin, const uint16_t* cos, bool chained,
+                    cudaStream_t stream) {
     EXL2B_CUDA(cudaSetDevice(a->device));
     const exl2b_qattn_desc& d = a->d;
     const int rows = batch * q_len;
     const bool rope = d.rope_style != 0 && sin;
     if (d.rope_style != 0 && rows > 1) EXL2B_REQUIRE(sin && cos, "rope needs sin/cos tables");
-    rc = qkv_stage(a, x, batch, q_len, past_len, past_lens, q, k, v, sin, cos, false, true, stream);
+    int rc = qkv_stage(a, x, batch, q_len, past_len, past_lens, q, k, v, sin, cos, chained, true, stream);
     if (rc) return rc;
+    lp.one_row = chained && !rope;
     lp.x = (const half*)x;
     lp.ldx = lp.K = d.hidden_size;
     lp.rows = rows;
@@ -570,6 +624,68 @@ extern "C" int exl2b_qattn_forward_1_lora(exl2b_qattn_t h, const uint16_t* x, in
         lp.neox = d.rope_style == 2;
     }
     return lora_launch(a->device, stream, lp);
+}
+
+extern "C" int exl2b_qattn_forward_1_lora(exl2b_qattn_t h, const uint16_t* x, int batch, int q_len, int past_len,
+                                          const int32_t* past_lens, uint16_t* q, uint16_t* k, uint16_t* v, const uint16_t* sin,
+                                          const uint16_t* cos, const uint64_t* ids, int num_ids, exl2b_stream_t stream) {
+    QAttn* a = (QAttn*)h;
+    EXL2B_REQUIRE(a && x && q && k && v && (ids || num_ids == 0), "null argument");
+    LoraParams lp = {};
+    int rc = lora_stack(a->loras, ids, num_ids, ATTN_STAGES[0], 3, lp);
+    if (rc) return rc;
+    if (lp.nseg == 0) return exl2b_qattn_forward_1(h, x, batch, q_len, past_len, past_lens, q, k, v, sin, cos, stream);
+    return qkv_lora(a, lp, x, batch, q_len, past_len, past_lens, q, k, v, sin, cos, false, (cudaStream_t)stream);
+}
+
+extern "C" int exl2b_qattn_forward_1_ex_lora(exl2b_qattn_t h, const uint16_t* x, int batch, int q_len, int past_len,
+                                             const int32_t* past_lens, uint16_t* q, uint16_t* k, uint16_t* v, const uint16_t* sin,
+                                             const uint16_t* cos, int input_prepared, const uint64_t* ids, int num_ids,
+                                             exl2b_stream_t stream) {
+    QAttn* a = (QAttn*)h;
+    EXL2B_REQUIRE(a && q && k && v && (ids || num_ids == 0), "null argument");
+    LoraParams lp = {};
+    int rc = lora_stack(a->loras, ids, num_ids, ATTN_STAGES[0], 3, lp);
+    if (rc) return rc;
+    if (lp.nseg == 0)
+        return exl2b_qattn_forward_1_ex(h, x, batch, q_len, past_len, past_lens, q, k, v, sin, cos, input_prepared, stream);
+    if (!input_prepared)
+        return exl2b_qattn_forward_1_lora(h, x, batch, q_len, past_len, past_lens, q, k, v, sin, cos, ids, num_ids, stream);
+    const QMatrix* qkv[3] = {(const QMatrix*)a->d.q_proj, (const QMatrix*)a->d.k_proj, (const QMatrix*)a->d.v_proj};
+    rc = lora_chain_rule(batch * q_len, row_path(batch * q_len, qkv, 3, a->i8_qkv, true));
+    if (rc) return rc;
+    EXL2B_REQUIRE(x, "LoRA adapters on a chained q|k|v: the LoRA launch reads the block input x, which the producer also leaves there");
+    return qkv_lora(a, lp, x, batch, q_len, past_len, past_lens, q, k, v, sin, cos, true, (cudaStream_t)stream);
+}
+
+extern "C" int exl2b_qattn_forward_2_ex_lora(exl2b_qattn_t h, uint16_t* x, const uint16_t* attn_out, int batch, int q_len,
+                                             int input_prepared, const exl2b_chain_t* next, const uint64_t* ids, int num_ids,
+                                             exl2b_stream_t stream) {
+    QAttn* a = (QAttn*)h;
+    EXL2B_REQUIRE(a && x && (ids || num_ids == 0), "null argument");
+    LoraParams lp = {};
+    int rc = lora_stack(a->loras, ids, num_ids, ATTN_STAGES[1], 1, lp);
+    if (rc) return rc;
+    if (lp.nseg == 0) return exl2b_qattn_forward_2_ex(h, x, attn_out, batch, q_len, input_prepared, next, stream);
+    if (!input_prepared && !(next && next->num_consumers > 0))
+        return exl2b_qattn_forward_2_lora(h, x, attn_out, batch, q_len, ids, num_ids, stream);
+    EXL2B_REQUIRE(a->d.o_proj, "this attention handle was created without o_proj");
+    const QMatrix* mo = (const QMatrix*)a->d.o_proj;
+    rc = lora_chain_rule(batch * q_len, row_path(batch * q_len, &mo, 1, mo->v.layout == LAYOUT_TC, true));
+    if (rc) return rc;
+    EXL2B_REQUIRE(attn_out, "LoRA adapters on a chained o_proj: the LoRA launch reads attn_out, which attention also writes");
+    rc = exl2b_qattn_forward_2_ex(h, x, attn_out, batch, q_len, input_prepared, next, stream);
+    if (rc) return rc;
+    lp.x = (const half*)attn_out;
+    lp.ldx = lp.K = mo->v.K;
+    lp.rows = 1;
+    lp.y[0] = (half*)x;
+    lp.n[0] = lp.ldy[0] = mo->v.N;
+    lp.epi = LORA_ADD;
+    lp.one_row = 1;
+    rc = lora_mirror(lp, 0, next);
+    if (rc) return rc;
+    return lora_launch(a->device, (cudaStream_t)stream, lp);
 }
 
 extern "C" int exl2b_qattn_forward_2_lora(exl2b_qattn_t h, uint16_t* x, const uint16_t* attn_out, int batch, int q_len,
@@ -647,4 +763,25 @@ extern "C" int exl2b_qmlp_forward_lora(exl2b_qmlp_t h, uint16_t* x, int rows, ui
     dn.n[0] = dn.ldy[0] = d.hidden_size;
     dn.epi = LORA_ADD;
     return lora_launch(m->device, stream, dn);
+}
+
+extern "C" int exl2b_qmlp_forward_ex_lora(exl2b_qmlp_t h, uint16_t* x, int rows, uint16_t* temp_a, uint16_t* temp_b,
+                                          int input_prepared, const exl2b_chain_t* next, const uint64_t* ids, int num_ids,
+                                          exl2b_stream_t stream) {
+    QMlp* m = (QMlp*)h;
+    EXL2B_REQUIRE(m && x && temp_a && (ids || num_ids == 0), "null argument");
+    EXL2B_REQUIRE(m->d.down, "this MLP handle was created without down_proj");
+    LoraParams gu = {}, dn = {};
+    int rc = lora_stack(m->loras, ids, num_ids, MLP_STAGES[0], 2, gu);
+    if (!rc) rc = lora_stack(m->loras, ids, num_ids, MLP_STAGES[1], 1, dn);
+    if (rc) return rc;
+    if (gu.nseg == 0 && dn.nseg == 0) return exl2b_qmlp_forward_ex(h, x, rows, temp_a, temp_b, input_prepared, next, stream);
+    if (!input_prepared && !(next && next->num_consumers > 0))
+        return exl2b_qmlp_forward_lora(h, x, rows, temp_a, temp_b, ids, num_ids, stream);
+    const QMatrix* dm = (const QMatrix*)m->d.down;
+    const QMatrix* gud[3] = {(const QMatrix*)m->d.gate, (const QMatrix*)m->d.up, dm};
+    rc = lora_chain_rule(rows, row_path(rows, gud, 3, m->i8_gu && dm->v.layout == LAYOUT_TC, true));
+    if (rc) return rc;
+    EXL2B_CUDA(cudaSetDevice(m->device));
+    return mlp_row(m, x, temp_a, temp_b, input_prepared, next, &gu, &dn, (cudaStream_t)stream);
 }

@@ -11,6 +11,11 @@
 //      of all clusters hold the same t = norm(x)·A;
 //   3. each CTA applies its share of the stacked B columns, t·B, to the base GEMMs' outputs and finishes them: the residual stream
 //      (o, down), RoPE of q and k (q|k|v), act(gate)·up (gate|up).
+// The one-row form (LoraParams::one_row) serves the chained single-row decode step (blocks.cu, the _ex_lora forms): there the
+// base launches write each output twice, as a plain row and as a copy in the next consumer's stored-row order, and every
+// consumer forms RMSNorm, RoPE and act·mul itself.  So the LoRA launch only adds the deltas, to the plain row and to that copy
+// (the mirror), and phase 3 spreads the columns over every CTA with 16-byte loads of B.  Down's input then is act(gate)·up
+// formed from the two plain rows (LoraParams::x2).  A's rows and B's columns are requested into L2 before the dependency wait.
 // Clusters split the output columns and recompute the small x·A from L2.  No global scratch, no atomics: the result is
 // deterministic, and the adapter list travels by value in the kernel parameters, so the launch can be captured in a graph.
 // All active adapters of a projection are summed in fp32 and y is rounded once (the reference rounds x·A to fp16 and y after
@@ -34,6 +39,42 @@ constexpr int LORA_SMEM_MAX = 184 * 1024;       // staged input rows of a CTA's 
 // adapter columns are stacked in groups of 8 (one 16-byte row segment of A per load): offsets and the bound count whole groups
 __host__ __device__ inline int rank_slots(int rank) { return (rank + 7) & ~7; }
 
+// outputs of a one-row launch: q, k, v / gate, up / the residual stream
+__host__ __device__ inline int lora_outputs(int epi) { return epi == LORA_QKV ? 3 : epi == LORA_ADD_PAIR ? 2 : 1; }
+
+// [p, p + bytes) into L2 at normal priority (the weights the GEMVs stream meanwhile are evict-first), shrunk to whole 16-byte
+// units inside the range
+__device__ __forceinline__ void prefetch_l2(const void* p, size_t bytes) {
+    const uintptr_t a = ((uintptr_t)p + 15) & ~(uintptr_t)15, e = ((uintptr_t)p + bytes) & ~(uintptr_t)15;
+    if (e > a) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(a), "r"((uint32_t)(e - a)) : "memory");
+}
+
+// one-row form: this CTA's groups [g0, g1) of 8 output columns, numbered over the launch's outputs in order
+__device__ __forceinline__ void one_row_groups(const LoraParams& P, int& g0, int& g1) {
+    const int gpc = (P.groups + (int)gridDim.x - 1) / (int)gridDim.x;
+    g0 = min(P.groups, (int)blockIdx.x * gpc);
+    g1 = min(P.groups, g0 + gpc);
+}
+
+// one-row form: the rows of B this CTA's columns read, one L2 prefetch per (segment, rank row) where B's rows are 16-byte aligned
+__device__ void lora_prefetch_b(const LoraParams& P, int tid) {
+    int g0, g1;
+    one_row_groups(P, g0, g1);
+    for (int p = 0, first = 0; p < lora_outputs(P.epi); ++p) {
+        const int n = P.n[p], gp = (n + 7) >> 3;
+        const int c0 = max(g0 - first, 0) * 8, c1 = min(min(g1 - first, gp) * 8, n);
+        first += gp;
+        if (c1 <= c0 || (n & 7)) continue;
+        for (int s = 0; s < P.nseg; ++s) {
+            const LoraSeg& sg = P.seg[s];
+            if (sg.proj != p) continue;
+            for (int j = tid; j < sg.rank; j += LORA_THREADS) prefetch_l2(sg.b + (size_t)j * n + c0, (size_t)(c1 - c0) * sizeof(half));
+        }
+    }
+}
+
+// ONE_ROW: LoraParams::one_row (a separate instantiation, so the un-chained form's code carries none of the one-row branches)
+template <bool ONE_ROW>
 __global__ void __launch_bounds__(LORA_THREADS) lora_kernel(const __grid_constant__ LoraParams P) {
     extern __shared__ float xs[];                          // [mt][len]: this CTA's K slice of the tile's input rows
     __shared__ float part[LORA_MT * LORA_MAX_RANK];        // this CTA's x·A over its slice, read by the whole cluster
@@ -49,6 +90,15 @@ __global__ void __launch_bounds__(LORA_THREADS) lora_kernel(const __grid_constan
     const int kper = ((P.K + cs - 1) / cs + 7) & ~7;
     const int k0 = min(P.K, cr * kper), len = min(P.K, k0 + kper) - k0;
 
+    // ---- 0. one-row form: the static operands, requested into L2 while the predecessor still runs: this CTA's rows of A and
+    //      its columns of B ---------------------------------------------------------------------------------------------------------
+    if constexpr (ONE_ROW) {
+        if (tid < P.nseg) {
+            const LoraSeg& sg = P.seg[tid];
+            prefetch_l2(sg.a + (size_t)k0 * sg.rank, (size_t)len * sg.rank * sizeof(half));
+        }
+        lora_prefetch_b(P, tid);
+    }
     griddep_launch_dependents();
     griddep_wait();
 
@@ -59,8 +109,11 @@ __global__ void __launch_bounds__(LORA_THREADS) lora_kernel(const __grid_constan
         ss[m] = 0.f;
         if (m < mt) {
             const half* xr = P.x + (size_t)(row0 + m) * P.ldx + k0;
+            const half* x2r = ONE_ROW && P.x2 ? P.x2 + (size_t)(row0 + m) * P.ldx + k0 : nullptr;
             for (int k = tid; k < len; k += LORA_THREADS) {
-                float f = __half2float(xr[k]);
+                float f;
+                if (ONE_ROW && P.x2) f = __half2float(__hmul(P.gelu ? gelu1(xr[k]) : __low2half(silu2(__half2half2(xr[k]))), x2r[k]));
+                else f = __half2float(xr[k]);
                 ss[m] = fmaf(f, f, ss[m]);
                 if (P.norm_w) f *= __half2float(P.norm_w[k0 + k]);
                 xs[m * len + k] = f;
@@ -161,6 +214,65 @@ __global__ void __launch_bounds__(LORA_THREADS) lora_kernel(const __grid_constan
         t_s[i] = s * rs_s[i / R];
     }
     cluster.sync();           // t_s complete; no CTA leaves while another still reads its partials
+
+    // ---- 3, one-row form: groups of 8 columns, the rank rows of a group split between tpg adjacent lanes (16-byte loads of B),
+    //      reduced by shuffles; the group's columns finished by its lanes in turn, each value stored to y and to its mirror -------
+    if constexpr (ONE_ROW) {
+        const int tpg = P.tpg;
+        int g0, g1;
+        one_row_groups(P, g0, g1);
+        for (int base = 0; base < (g1 - g0) * tpg; base += LORA_THREADS) {      // the same trip count in every thread
+            const int w = base + tid, g = g0 + w / tpg, sub = w & (tpg - 1);
+            float d[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) d[e] = 0.f;
+            int p = 0, c = 0;
+            if (g < g1) {
+                int gg = g;
+                while (p < lora_outputs(P.epi) - 1 && gg >= (P.n[p] + 7) >> 3) gg -= (P.n[p++] + 7) >> 3;
+                c = gg * 8;
+                const int n = P.n[p];
+                for (int s = 0, f0 = 0; s < P.nseg; ++s) {
+                    const LoraSeg& sg = P.seg[s];
+                    if (sg.proj != p) continue;
+                    const half* b = sg.b + c;
+                    const bool vec = (n & 7) == 0 && ((uintptr_t)sg.b & 15) == 0;
+#pragma unroll 2
+                    for (int j = (sub - f0) & (tpg - 1); j < sg.rank; j += tpg) {      // rank row f0 + j of the projection: lane sub
+                        const float t = t_s[sg.off + j];
+                        if (vec) {
+                            const uint4 v = ldg_ef(reinterpret_cast<const uint4*>(b + (size_t)j * n));
+                            const half2* h = reinterpret_cast<const half2*>(&v);
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) {
+                                d[2 * i] = fmaf(t, __low2float(h[i]), d[2 * i]);
+                                d[2 * i + 1] = fmaf(t, __high2float(h[i]), d[2 * i + 1]);
+                            }
+                        } else {
+#pragma unroll
+                            for (int e = 0; e < 8; ++e)
+                                if (c + e < n) d[e] = fmaf(t, __half2float(b[(size_t)j * n + e]), d[e]);
+                        }
+                    }
+                    f0 += sg.rank;
+                }
+            }
+            for (int o = tpg >> 1; o > 0; o >>= 1)
+#pragma unroll
+                for (int e = 0; e < 8; ++e) d[e] += __shfl_xor_sync(0xffffffffu, d[e], o);
+            if (g >= g1) continue;
+            half* y = P.y[p];
+            half* mir = P.mirror[p];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                if ((e & (tpg - 1)) != sub || c + e >= P.n[p]) continue;
+                const half v = __float2half_rn(__half2float(y[c + e]) + d[e]);
+                y[c + e] = v;
+                if (mir) mir[P.mirror_invperm[p][c + e]] = v;
+            }
+        }
+        return;
+    }
 
     // ---- 3. t·B on this CTA's units of output columns, then the stage's epilogue -------------------------------------------------
     const int ctas = gridDim.x, upc = (P.units + ctas - 1) / ctas;
@@ -325,13 +437,31 @@ int lora_take(const exl2b_lora_t* loras, int num, const int* ks, const int* ns, 
 
 int lora_launch(int device, cudaStream_t stream, LoraParams& p) {
     if (p.nseg == 0 || p.rows <= 0) return 0;
-    if (p.epi == LORA_QKV) {
+    int clusters = 0;
+    if (p.one_row) {
+        EXL2B_REQUIRE(p.rows == 1 && !p.sin && p.epi != LORA_ACT_MUL, "LoRA: the one-row form takes one row, no RoPE and no act·mul");
+        // groups of 8 columns over up to one wave of CTAs; lanes per group while a CTA's groups fill its threads, at most the
+        // largest summed rank of one projection
+        p.groups = 0;
+        int rmax = 0;
+        for (int o = 0; o < lora_outputs(p.epi); ++o) {
+            p.groups += (p.n[o] + 7) / 8;
+            int r = 0;
+            for (int s = 0; s < p.nseg; ++s) r += p.seg[s].proj == o ? p.seg[s].rank : 0;
+            rmax = std::max(rmax, r);
+        }
+        clusters = std::max(1, std::min(LORA_MAX_CTAS / LORA_CLUSTER, (p.groups + LORA_CLUSTER - 1) / LORA_CLUSTER));
+        const int gpc = (p.groups + clusters * LORA_CLUSTER - 1) / (clusters * LORA_CLUSTER);
+        p.tpg = 1;
+        while (p.tpg < 32 && p.tpg < rmax && 2 * p.tpg * gpc <= LORA_THREADS) p.tpg *= 2;
+    } else if (p.epi == LORA_QKV) {
         p.unit_pairs = p.head_dim / 2;
         p.units = p.heads_q + 2 * p.heads_kv;
     } else if (p.epi == LORA_ACT_MUL) {
         p.unit_pairs = 64;
         p.units = (p.n[0] + 63) / 64;
     } else {
+        EXL2B_REQUIRE(p.epi == LORA_ADD, "LoRA: epilogue %d needs the one-row form", p.epi);
         EXL2B_REQUIRE(p.n[0] % 2 == 0, "LoRA: output width %d is odd", p.n[0]);
         p.unit_pairs = 32;
         p.units = (p.n[0] + 63) / 64;
@@ -344,12 +474,13 @@ int lora_launch(int device, cudaStream_t stream, LoraParams& p) {
                   LORA_SMEM_MAX);
     static bool attr_set[64] = {};
     if (!attr_set[device]) {
-        EXL2B_CUDA(cudaFuncSetAttribute(lora_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LORA_SMEM_MAX));
+        EXL2B_CUDA(cudaFuncSetAttribute(lora_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, LORA_SMEM_MAX));
+        EXL2B_CUDA(cudaFuncSetAttribute(lora_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, LORA_SMEM_MAX));
         attr_set[device] = true;
     }
     // clusters over the output units: up to one wave of CTAs in all, fewer when there are many row tiles
     const int want = (p.units + LORA_CLUSTER - 1) / LORA_CLUSTER;
-    const int clusters = std::max(1, std::min(want, LORA_MAX_CTAS / LORA_CLUSTER / tiles));
+    if (!p.one_row) clusters = std::max(1, std::min(want, LORA_MAX_CTAS / LORA_CLUSTER / tiles));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(clusters * LORA_CLUSTER, tiles);
     cfg.blockDim = dim3(LORA_THREADS);
@@ -365,7 +496,7 @@ int lora_launch(int device, cudaStream_t stream, LoraParams& p) {
     cfg.attrs = attr;
     cfg.numAttrs = pdl_disabled("lora") ? 1 : 2;
     g_launch_count.fetch_add(1, std::memory_order_relaxed);
-    EXL2B_CUDA(cudaLaunchKernelEx(&cfg, lora_kernel, p));
+    EXL2B_CUDA(p.one_row ? cudaLaunchKernelEx(&cfg, lora_kernel<true>, p) : cudaLaunchKernelEx(&cfg, lora_kernel<false>, p));
     return 0;
 }
 

@@ -35,6 +35,7 @@ enum LoraEpilogue : int {
     LORA_ADD = 0,       // y[0] += delta                                            (o, down: the residual stream)
     LORA_QKV = 1,       // y[p] += delta for q, k, v; then RoPE on q and k          (rope_kernel arithmetic)
     LORA_ACT_MUL = 2,   // act_out = act(y[0] + delta_gate) * (y[1] + delta_up)   (act_mul_kernel arithmetic)
+    LORA_ADD_PAIR = 3,  // y[0] += delta_gate, y[1] += delta_up, nothing more      (one-row form: down's prologue forms act·mul)
 };
 
 struct LoraParams {
@@ -55,7 +56,17 @@ struct LoraParams {
     int past_len, q_len, head_dim, sincos_size, neox, heads_q, heads_kv;
     // LORA_ACT_MUL
     half* act_out;
-    int ld_act, gelu;
+    int ld_act, gelu;            // gelu: also the activation of the x2 input below
+    // input act(x) * x2 (x2 != NULL): the input row formed from the plain gate and up rows with I8_SILU_MUL / I8_GELU_MUL's fp16
+    // operations (down's input in the chained single-row step, where the act·mul row never exists in memory)
+    const half* x2;
+    // one-row form (one_row = 1, rows = 1, no RoPE, epilogue ADD / QKV / ADD_PAIR): phase 3 spreads the stage's output columns
+    // over all CTAs in groups of 8 (`groups` in all, set by lora_launch), each group's rank rows split between `tpg` threads
+    // that read B 16 bytes at a time.  Every finished y[p][n] is also stored, same bits, at mirror[p][mirror_invperm[p][n]]
+    // when mirror[p] is given: the copy a chained producer leaves in its consumer's stored-row order (I8Out::c_perm).
+    int one_row, groups, tpg;
+    half* mirror[3];
+    const uint16_t* mirror_invperm[3];
 };
 
 // Stack the adapters of `ids` that have a projection in `projs` into p.seg (ids with none are skipped); -2 past the bounds.

@@ -119,6 +119,12 @@ _sig("exl2b_qattn_forward_1_lora", c_int, c_void_p, c_void_p, c_int, c_int, c_in
      c_void_p, c_void_p, POINTER(c_uint64), c_int, c_void_p)
 _sig("exl2b_qattn_forward_2_lora", c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(c_uint64), c_int, c_void_p)
 _sig("exl2b_qmlp_forward_lora", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, POINTER(c_uint64), c_int, c_void_p)
+_sig("exl2b_qattn_forward_1_ex_lora", c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+     c_void_p, c_void_p, c_int, POINTER(c_uint64), c_int, c_void_p)
+_sig("exl2b_qattn_forward_2_ex_lora", c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(_Chain), POINTER(c_uint64),
+     c_int, c_void_p)
+_sig("exl2b_qmlp_forward_ex_lora", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, POINTER(_Chain), POINTER(c_uint64),
+     c_int, c_void_p)
 _sig("exl2b_lora_stack", c_int, POINTER(c_int), c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int),
      POINTER(c_int))
 
@@ -656,21 +662,38 @@ def make_chain(consumers, norm_weight=None) -> "_Chain":
 
 
 def q_attn_forward_1_ex(q_attn: int, x, batch_size: int, q_len: int, past_len: int, past_lens, q_temp, k_temp, v_temp, sin, cos,
-                        input_prepared: bool):
+                        input_prepared: bool, loras=()):
+    """loras: active adapter ids (as q_attn_forward_1); a chained call with adapters takes one row (include/exl2_b200.h _ex_lora)"""
+    if loras:
+        ids, n = _lora_ids(loras)
+        _check(lib.exl2b_qattn_forward_1_ex_lora(q_attn, _p(x), batch_size, q_len, int(past_len), _p(past_lens), q_temp.data_ptr(),
+                                                 k_temp.data_ptr(), v_temp.data_ptr(), _p(sin), _p(cos), int(input_prepared), ids, n,
+                                                 _stream(q_temp)))
+        return
     _check(lib.exl2b_qattn_forward_1_ex(q_attn, _p(x), batch_size, q_len, int(past_len), _p(past_lens), q_temp.data_ptr(),
                                         k_temp.data_ptr(), v_temp.data_ptr(), _p(sin), _p(cos), int(input_prepared), _stream(q_temp)))
 
 
-def q_attn_forward_2_ex(q_attn: int, x, attn_output, batch_size: int, q_len: int, input_prepared: bool, chain=None):
-    _check(lib.exl2b_qattn_forward_2_ex(q_attn, x.data_ptr(), _p(attn_output), batch_size, q_len, int(input_prepared),
-                                        ctypes.byref(chain) if chain is not None else None, _stream(x)))
+def q_attn_forward_2_ex(q_attn: int, x, attn_output, batch_size: int, q_len: int, input_prepared: bool, chain=None, loras=()):
+    ch = ctypes.byref(chain) if chain is not None else None
+    if loras:
+        ids, n = _lora_ids(loras)
+        _check(lib.exl2b_qattn_forward_2_ex_lora(q_attn, x.data_ptr(), _p(attn_output), batch_size, q_len, int(input_prepared), ch,
+                                                 ids, n, _stream(x)))
+        return
+    _check(lib.exl2b_qattn_forward_2_ex(q_attn, x.data_ptr(), _p(attn_output), batch_size, q_len, int(input_prepared), ch, _stream(x)))
 
 
-def q_mlp_forward_ex(q_mlp: int, x, input_prepared: bool, chain=None):
+def q_mlp_forward_ex(q_mlp: int, x, input_prepared: bool, chain=None, loras=()):
     temp_a, temp_b = _mlp_temps[q_mlp]
     rows = x.numel() // x.shape[-1]
-    _check(lib.exl2b_qmlp_forward_ex(q_mlp, x.data_ptr(), rows, temp_a.data_ptr(), _p(temp_b), int(input_prepared),
-                                     ctypes.byref(chain) if chain is not None else None, _stream(x)))
+    ch = ctypes.byref(chain) if chain is not None else None
+    if loras:
+        ids, n = _lora_ids(loras)
+        _check(lib.exl2b_qmlp_forward_ex_lora(q_mlp, x.data_ptr(), rows, temp_a.data_ptr(), _p(temp_b), int(input_prepared), ch,
+                                              ids, n, _stream(x)))
+        return
+    _check(lib.exl2b_qmlp_forward_ex(q_mlp, x.data_ptr(), rows, temp_a.data_ptr(), _p(temp_b), int(input_prepared), ch, _stream(x)))
 
 
 def gemm_half_q_half_prepared(b: int, c, has_norm: bool, norm_eps: float, clear: bool = True):

@@ -341,11 +341,16 @@ class ExLlamaV2Decoder:
         more rows only when every matrix can be staged by the wgmma kernel (otherwise the blocks take the dense path): up to 8
         rows in any step, and a decode step (one new token per sequence) of 17..32 sequences on the 32-row wgmma tile, which
         reads the packed weights once where the un-chained step reconstructs every matrix.  Above 32 sequences the 64-row tile
-        measured slower than the dense path on the 7B preset (DESIGN.md §7), so those steps stay un-chained.  Never with active
-        adapters: their deltas need each stage's raw outputs in memory (the un-chained block forms)."""
+        measured slower than the dense path on the 7B preset (DESIGN.md §7), so those steps stay un-chained.  With active
+        adapters only one row on the integer GEMV: there each launch leaves its output as a plain row plus a copy for its consumer,
+        which forms RMSNorm, RoPE and act·mul itself, so a LoRA launch after it can add the deltas to both (include/exl2_b200.h
+        _ex_lora).  Above one row the chained launches fuse RoPE, act·mul and the RMSNorm sums into their epilogues, where no
+        delta can be added after them, so adapted steps stay on the un-chained block forms."""
         wide = q_len == 1 and GEMM_BIG_MIN_ROWS < rows <= DECODE_CHAIN_ROWS
-        if not (self.chained and self.fused_attn and (rows <= 8 or wide)) or self.lora_ids:
+        if not (self.chained and self.fused_attn and (rows <= 8 or wide)):
             return False
+        if self.lora_ids:
+            return rows == 1 and self.row_gemv
         return self.tc_staged or (rows == 1 and self.row_gemv)
 
     @property
@@ -399,25 +404,25 @@ class ExLlamaV2Decoder:
         fuse_rope = self.row_gemv and B * q_len == 1
         for li, L in enumerate(self.layers):
             ext_c.q_attn_forward_1_ex(L.attn, x, B, q_len, -1, cache.cache_seqlens, q, k, v,
-                                      None if fuse_rope else self.sin, None if fuse_rope else self.cos, li > 0)
+                                      None if fuse_rope else self.sin, None if fuse_rope else self.cos, li > 0, self.lora_ids)
             if not gemv_only:        # (bench.py's roofline loop replays exactly the GEMV launches, nothing else)
                 ext_c.paged_attn_decode_q4(q.view(B, q_len, H, hd), k.view(B, q_len, KVH, hd), v.view(B, q_len, KVH, hd),
                                            cache.key_states[li], cache.key_scales[li], cache.value_states[li],
                                            cache.value_scales[li], cache.cache_seqlens, cache.block_table,
                                            attn_out.view(B, q_len, H, hd), 1.0 / math.sqrt(hd), L.o_proj.q_handle,
                                            rope=(self.sin, self.cos, 2) if fuse_rope else None, wbits=cache.wbits)
-            ext_c.q_attn_forward_2_ex(L.attn, x, attn_out, B, q_len, True, L.chain_mlp)
+            ext_c.q_attn_forward_2_ex(L.attn, x, attn_out, B, q_len, True, L.chain_mlp, self.lora_ids)
             if li + 1 < n:
                 nxt = self.layers[li + 1].chain_attn
             else:
                 nxt = self.chain_head if head else None
-            ext_c.q_mlp_forward_ex(L.mlp, x, True, nxt)
+            ext_c.q_mlp_forward_ex(L.mlp, x, True, nxt, self.lora_ids)
         if not gemv_only:
             cache.cache_seqlens.add_(q_len)
 
     def _decode_step(self):
         torch.index_select(self.embed, 0, self.ids.view(-1), out=self.x.view(self.batch_size, -1))
-        if self.row_gemv and self.batch_size == 1 and self.chained and self.fused_attn and not self.lora_ids:
+        if self.row_gemv and self.batch_size == 1 and self.chained and self.fused_attn:
             self._forward_tokens_chained(self.x, self.q, self.k, self.v, self.attn_out, 1, head=True)
             ext_c.gemv_norm(self.x.view(1, -1), self.lm_head.q_handle, self.final_norm, self.cfg.norm_eps, self.logits, prepared=True)
             return

@@ -324,6 +324,27 @@ int exl2b_qattn_forward_2_ex(exl2b_qattn_t h, uint16_t* x, const uint16_t* attn_
                              const exl2b_chain_t* next, exl2b_stream_t stream);
 int exl2b_qmlp_forward_ex(exl2b_qmlp_t h, uint16_t* x, int rows, uint16_t* temp_a, uint16_t* temp_b, int input_prepared,
                           const exl2b_chain_t* next, exl2b_stream_t stream);
+/* The chained forms with the call's active adapter ids (as the _lora forms above).  When no id has an adapter on the call's
+ * stages, the call is exactly the _ex call.  An un-chained call (input_prepared = 0 and no `next`) is exactly the _lora call.
+ * A chained call with adapters runs each adapted stage as its chained base launch(es) followed by ONE LoRA launch in the
+ * one-row form (csrc/lora.cu): it adds the deltas to the plain output row AND to the copy the base launch left in the next
+ * consumer's stored-row order (the mirror), with the same bits, so the consumer reads the adapted row:
+ *   q|k|v   q, k, v (no mirror: attention reads the plain rows; with sin / cos given the launch also applies RoPE);
+ *   o       x, mirrored into next's first consumer (gate);
+ *   gate|up the plain gate row (temp_a) and up row (temp_b), mirrored into down's input slots; no act·mul, down's prologue
+ *           forms it;
+ *   down    x, mirrored into next's first consumer (the next layer's q, or lm_head); its input act(gate)·up is formed from the
+ *           two plain rows with the fp16 operations of down's own prologue.
+ * The LoRA launches read x (q|k|v, gate|up) and attn_out (o) as plain rows in feature order, so neither may be NULL.  This holds
+ * at ONE row on the integer GEMV only: above one row the chained launches fuse RoPE, act·mul and the RMSNorm sums of squares
+ * into their epilogues, so no delta can be added after them -- such a call with an active adapter fails, saying so. */
+int exl2b_qattn_forward_1_ex_lora(exl2b_qattn_t h, const uint16_t* x, int batch, int q_len, int past_len, const int32_t* past_lens,
+                                  uint16_t* q, uint16_t* k, uint16_t* v, const uint16_t* sin, const uint16_t* cos,
+                                  int input_prepared, const uint64_t* ids, int num_ids, exl2b_stream_t stream);
+int exl2b_qattn_forward_2_ex_lora(exl2b_qattn_t h, uint16_t* x, const uint16_t* attn_out, int batch, int q_len, int input_prepared,
+                                  const exl2b_chain_t* next, const uint64_t* ids, int num_ids, exl2b_stream_t stream);
+int exl2b_qmlp_forward_ex_lora(exl2b_qmlp_t h, uint16_t* x, int rows, uint16_t* temp_a, uint16_t* temp_b, int input_prepared,
+                               const exl2b_chain_t* next, const uint64_t* ids, int num_ids, exl2b_stream_t stream);
 /* gemm_half_q_half on an input prepared by a chained producer (lm_head after the last MLP; has_norm: apply 1/rms) */
 int exl2b_gemm_half_q_half_prepared(exl2b_qmatrix_t h, uint16_t* c, int ldc, int m, int clear, int has_norm, float norm_eps,
                                     exl2b_stream_t stream);

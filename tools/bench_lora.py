@@ -2,9 +2,10 @@
 
     python tools/bench_lora.py [--model llama2-7b-4.0bpw] [--steps 64] [--warmup 8] [--rounds 5] [--out DIR]
 
-Configurations, alternated within one process round by round so that they see the same machine: no adapter; no adapter on the
-un-chained schedule that a step with adapters runs; rank 16 on q and v (the common PEFT target); rank 16 on all seven
-projections; rank 64 on all seven.  Workloads: batch-1 and batch-8 decode
+Configurations, alternated within one process round by round so that they see the same machine: no adapter; rank 16 on q and v
+(the common PEFT target); rank 16 on all seven projections; rank 64 on all seven -- each also on the un-chained schedule
+(`dec.chained = False`, the "-unchained" rows), which is what a step with adapters ran before batch-1 steps could chain them,
+and what steps of more than one row with adapters still run.  Workloads: batch-1 and batch-8 decode
 (ExLlamaV2Decoder.decode replaying the captured step), and prefill_rows of 16 sequences x 128 tokens (not captured: it
 allocates its activations per call).  Per configuration: tok/s as median [min, max] over the rounds, the library's launches per
 step (eager), the adapter bytes a token reads on top of the weights (A and B of every active projection, once per step / batch),
@@ -28,9 +29,13 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."
 from exllamav2_b200 import ext  # noqa: E402
 from exllamav2_b200.model import PRESETS, ExLlamaV2Decoder  # noqa: E402
 
-# "unchained": no adapter, but the un-chained schedule every step with adapters takes -- what the adapters cost beyond the schedule
-CONFIGS = {"none": None, "unchained": None, "qv-r16": (16, ("q_proj", "v_proj")), "all-r16": (16, ExLlamaV2Decoder.LORA_TARGETS),
-           "all-r64": (64, ExLlamaV2Decoder.LORA_TARGETS)}
+# name -> (adapter: (rank, targets) or None, chained schedule allowed).  "unchained": no adapter on the un-chained schedule; the
+# "-unchained" adapter rows beside their chained ones show what the schedule is worth with adapters
+_QV, _ALL = ("q_proj", "v_proj"), ExLlamaV2Decoder.LORA_TARGETS
+CONFIGS = {"none": (None, True), "unchained": (None, False),
+           "qv-r16": ((16, _QV), True), "qv-r16-unchained": ((16, _QV), False),
+           "all-r16": ((16, _ALL), True), "all-r16-unchained": ((16, _ALL), False),
+           "all-r64": ((64, _ALL), True), "all-r64-unchained": ((64, _ALL), False)}
 
 
 def card() -> str:
@@ -73,10 +78,10 @@ def bench_decode(cfg, B: int, args) -> dict:
         dec.cache.cache_seqlens.copy_(start)
         dec.pos = 0
 
-    for i, (name, c) in enumerate(CONFIGS.items()):
+    for i, (name, (c, chained)) in enumerate(CONFIGS.items()):
         key = dec.load_lora(c[0], targets=c[1], seed=i) if c else None
         dec.set_loras([key] if key else [])
-        dec.chained = name != "unchained"
+        dec.chained = chained
         torch.cuda.synchronize()
         n0 = ext.launch_count()
         dec.decode(ids)
@@ -124,10 +129,10 @@ def bench_prefill_rows(cfg, B: int, T: int, args) -> dict:
         dec.prefill_rows(ids, cache_attn=True)
 
     for r in range(args.rounds):
-        for i, (name, c) in enumerate(CONFIGS.items()):
+        for i, (name, (c, chained)) in enumerate(CONFIGS.items()):
             key = dec.load_lora(c[0], targets=c[1], seed=i) if c else None
             dec.set_loras([key] if key else [])
-            dec.chained = name != "unchained"          # (prefill_rows never chains: the same as "none")
+            dec.chained = chained          # (prefill_rows never chains: the same as "none")
             run()
             torch.cuda.synchronize()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -172,7 +177,7 @@ def main() -> None:
         for name, r in out[wl].items():
             t = r["tok_s"]
             extra = " ".join(f"{k}={v:.1f}" if isinstance(v, float) else f"{k}={v}" for k, v in r.items() if k != "tok_s")
-            print(f"{wl:22s} {name:8s} {t['median']:9.1f} tok/s [{t['min']:.1f}, {t['max']:.1f}]  {extra}")
+            print(f"{wl:22s} {name:17s} {t['median']:9.1f} tok/s [{t['min']:.1f}, {t['max']:.1f}]  {extra}")
     line = json.dumps(out)
     if args.out:
         os.makedirs(args.out, exist_ok=True)
