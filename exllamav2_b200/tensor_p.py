@@ -10,8 +10,12 @@ ext_qmlp.cpp:326-473, re-designed for one process per GPU:
   * the K/V cache is sharded by kv-head (cache.py:659-692): attention is rank-local.
   * a sharded activation is re-replicated with ONE all-gather (torch.distributed, NCCL over NVLink) where the reference
     stages through pinned host memory (ext_tp.cpp:129-293): after attention (rows x H*hd), after O-proj into the residual
-    stream, after act*mul (rows x intermediate), after down-proj -- 4 per layer + 1 for the logits.  No all-reduce: the
-    summation order of every output element is the single-GPU order, results are bit-identical to the unsharded run.
+    stream, after act*mul (rows x intermediate), after down-proj -- 4 per layer + 1 for the logits.  No all-reduce: every
+    output element is summed over the whole K on one rank.  On test-small's dimensions the results measured the same bits at
+    every world size, and they are the same bits as the un-chained single-GPU decoder wherever both issue the same launches
+    (calls of one sequence, and of more than 16 rows); where the single-GPU blocks fuse stages that a rank runs as separate launches
+    (several sequences at 2..16 rows), and in the hd-128 models' decode steps, the two agree to within their error against
+    fp64, not bit for bit (tests/test_gpu_tp_one_device.py).
   * the whole sharded decode step, collectives included, is captured in one CUDA graph per rank.
 
 At batch 1 these collectives are latency-bound (8-22 KB each); DESIGN.md discusses the peer-store epilogue that replaces
@@ -128,6 +132,7 @@ class ExLlamaV2DecoderTP:
         gen.manual_seed(seed)
         self.weight_bytes = 0
         self.layers, self.linears = [], []
+        max_rows = max(64, 8 * batch_size)          # rows of one call through the blocks (their temp_a): 8 tokens per sequence
 
         def lin(K, N, plan, s, cols, perm_seed=None):
             w = synthetic.random_linear(K, N, plan, device=dev, seed=s, weight_std=1.0 / math.sqrt(K), perm_seed=perm_seed)
@@ -158,14 +163,13 @@ class ExLlamaV2DecoderTP:
             s += 16
             L.input_norm = (1 + 0.1 * torch.randn((hid,), device=dev, generator=gen)).half()
             L.post_norm = (1 + 0.1 * torch.randn((hid,), device=dev, generator=gen)).half()
-            L.temp_a = torch.empty((64, self.inter_l), dtype=torch.half, device=dev)
-            L.temp_b = torch.empty((64, self.inter_l), dtype=torch.half, device=dev)
+            L.temp_a = torch.empty((max_rows, self.inter_l), dtype=torch.half, device=dev)
             # rank-local blocks: this rank's heads / intermediate columns; o_proj and down are applied as column shards below
             L.attn = ext_c.make_q_attn(L.input_norm, none_tensor, True, False, cfg.norm_eps, L.q_proj.q_handle, L.k_proj.q_handle,
-                                       L.v_proj.q_handle, 0, none_tensor, none_tensor, 64, hid, self.Hl, self.KVHl, hd,
+                                       L.v_proj.q_handle, 0, none_tensor, none_tensor, max_rows, hid, self.Hl, self.KVHl, hd,
                                        cfg.max_seq_len, True, 2, hd, none_tensor, none_tensor, none_tensor, none_tensor, False, True)
             L.mlp = ext_c.make_q_mlp(L.post_norm, none_tensor, True, cfg.norm_eps, L.gate.q_handle, L.up.q_handle, 0,
-                                     none_tensor, L.temp_a, none_tensor, none_tensor, 64, False, True, none_tensor, none_tensor,
+                                     none_tensor, L.temp_a, none_tensor, none_tensor, max_rows, False, True, none_tensor, none_tensor,
                                      False, True)
             self.layers.append(L)
         self.final_norm = (1 + 0.1 * torch.randn((hid,), device=dev, generator=gen)).half()
@@ -228,6 +232,7 @@ class ExLlamaV2DecoderTP:
             self.tp.all_gather_cols(self.logits, loc)
 
     def prefill(self, ids: torch.Tensor, chunk: int = 8):
+        """Feed a prompt [B, T], `chunk` tokens at a time; returns the last chunk's hidden state [B, n, hidden] (replicated)."""
         B, T = ids.shape
         hd = self.cfg.head_dim
         if self.pos + T > self.cache.max_seq_len:
@@ -239,6 +244,7 @@ class ExLlamaV2DecoderTP:
             q = torch.empty((B, n, self.Hl * hd), dtype=torch.half, device=self.device)
             k = torch.empty((B, n, self.KVHl * hd), dtype=torch.half, device=self.device)
             self._forward_rows(x, q, k, torch.empty_like(k), n)
+        return x.view(B, n, -1)
 
     def capture(self, body=None):
         body = body or self._decode_step
@@ -269,6 +275,14 @@ class ExLlamaV2DecoderTP:
         else:
             self._decode_step()
         return self.logits
+
+    def unload(self):
+        for L in self.layers:
+            self.ext.free_q_attn(L.attn)
+            self.ext.free_q_mlp(L.mlp)
+        for l in self.linears:
+            l.unload()
+        self.layers, self.linears = [], []
 
 
 # ---- bench.py --gpus N > 1 ------------------------------------------------------------------------------------------

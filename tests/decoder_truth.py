@@ -366,7 +366,7 @@ def as_starts(starts, B: int) -> np.ndarray:
     return np.full(B, int(a[0]), dtype=np.int64) if a.size == 1 else a
 
 
-def check_call(dec, truth, sched, kind, ids, out, pre, post, starts, chunk=8, floor_ratio=0.0, poison=None):
+def check_call(dec, truth, sched, kind, ids, out, pre, post, starts, chunk=8, floor_ratio=0.0, poison=None, allow=None, stats=None):
     """What every checked decoder call must satisfy, given the cache snapshots before (pre) and after (post) it and its output
     (decode: logits [B, vocab]; prompt: hidden state [B, T_last, hidden]).  starts: each sequence's position before the call
     (an int array [B], or one int for all); dec.pos, the host's mirror, must have advanced from max(starts):
@@ -376,7 +376,8 @@ def check_call(dec, truth, sched, kind, ids, out, pre, post, starts, chunk=8, fl
            or FLOOR_RATIO x that row's fp16 floor);
       (2c) with `poison` (poison_past), every poisoned byte the call did not append into unchanged;
       (1) the output per sequence within OUT_TOL[sched] rel-L2 of the truth, scaled up by floor / FLOOR_TYPICAL where this
-          input's fp16 floor is larger than that, and never below floor_ratio x the floor (0: off).
+          input's fp16 floor is larger than that, and never below floor_ratio x the floor (0: off) or allow[b] (None: off).
+    stats: a dict that receives the per-sequence output rel-L2 ("err") and fp16 floor ("floor").
     Returns (worst output rel-L2, worst floor, number of sequences whose bound was scaled)."""
     import kv_q68
     from exl2_oracle import rel_l2
@@ -416,7 +417,10 @@ def check_call(dec, truth, sched, kind, ids, out, pre, post, starts, chunk=8, fl
                                            f"{e[bad] / nt[bad]} vs quantisation {eq[bad] / nt[bad]}, fp16 floor {floor[bad] / nt[bad]}")
         want, want16 = (res.logits[-1], res16.logits[-1]) if kind == "decode" else (res.hidden, res16.hidden)
         err, floor = rel_l2(out[b], want), rel_l2(want16, want)
-        bound = max(OUT_TOL[sched] * max(1.0, floor / FLOOR_TYPICAL), floor_ratio * floor)
+        if stats is not None:
+            stats.setdefault("err", []).append(err)
+            stats.setdefault("floor", []).append(floor)
+        bound = max(OUT_TOL[sched] * max(1.0, floor / FLOOR_TYPICAL), floor_ratio * floor, 0.0 if allow is None else allow[b])
         floored += bound > OUT_TOL[sched]
         worst, worst_floor = max(worst, err), max(worst_floor, floor)
         assert err <= bound, (f"{sched} seq {b} (start {pos0}): rel-L2 {err:.3e} vs the fp64 truth (bound {bound:.3e}, "
