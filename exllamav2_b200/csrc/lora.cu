@@ -11,7 +11,7 @@
 //      of all clusters hold the same t = norm(x)·A;
 //   3. each CTA applies its share of the stacked B columns, t·B, to the base GEMMs' outputs and finishes them: the residual stream
 //      (o, down), RoPE of q and k (q|k|v), act(gate)·up (gate|up).
-// The one-row form (LoraParams::one_row) serves the chained single-row decode step (blocks.cu, the _ex_lora forms): there the
+// The one-row form (LoraParams::one_row) serves the chained single-row decode step (blocks.cu, chained adapted calls): there the
 // base launches write each output twice, as a plain row and as a copy in the next consumer's stored-row order, and every
 // consumer forms RMSNorm, RoPE and act·mul itself.  So the LoRA launch only adds the deltas, to the plain row and to that copy
 // (the mirror), and phase 3 spreads the columns over every CTA with 16-byte loads of B.  Down's input then is act(gate)·up

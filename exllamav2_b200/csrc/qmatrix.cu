@@ -293,7 +293,7 @@ static void fill_left_same(std::vector<uint2>& tab) {
 using namespace exl2b;
 
 extern "C" const char* exl2b_last_error(void) { return g_err; }
-extern "C" int exl2b_version(void) { return 100; }
+extern "C" int exl2b_version(void) { return 101; }
 extern "C" uint64_t exl2b_launch_count(void) { return g_launch_count.load(); }
 
 extern "C" int exl2b_make_group_map(const int16_t* q_groups, int num_groups, int num_qrows, int16_t* out,

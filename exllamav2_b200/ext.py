@@ -83,12 +83,8 @@ _sig("exl2b_fp16_to_q_kv", c_int, *_KV_ARGS)
 _sig("exl2b_q_to_fp16_kv", c_int, *_KV_ARGS)
 _sig("exl2b_qattn_create", c_int, POINTER(_QAttnDesc), POINTER(c_void_p))
 _sig("exl2b_qattn_destroy", c_int, c_void_p)
-_sig("exl2b_qattn_forward_1", c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-     c_void_p, c_void_p, c_void_p)
-_sig("exl2b_qattn_forward_2", c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p)
 _sig("exl2b_qmlp_create", c_int, POINTER(_QMlpDesc), POINTER(c_void_p))
 _sig("exl2b_qmlp_destroy", c_int, c_void_p)
-_sig("exl2b_qmlp_forward", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p)
 _sig("exl2b_qmlp_forward_gateup", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p)
 _sig("exl2b_paged_attn_decode_q", c_int, *([c_void_p] * 10 + [c_int] * 7 + [c_float, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]))
 _sig("exl2b_paged_attn_prefill_q", c_int, *([c_void_p] * 10 + [c_int] * 7 + [c_float, c_int, c_void_p]))
@@ -101,10 +97,13 @@ class _Chain(Structure):
     _fields_ = [("consumers", c_void_p * 3), ("num_consumers", c_int), ("norm_weight", c_void_p)]
 
 
-_sig("exl2b_qattn_forward_1_ex", c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-     c_void_p, c_void_p, c_int, c_void_p)
-_sig("exl2b_qattn_forward_2_ex", c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(_Chain), c_void_p)
-_sig("exl2b_qmlp_forward_ex", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, POINTER(_Chain), c_void_p)
+# the block forwards (include/exl2_b200.h "block forwards"): ..., input_prepared, next, ids, num_ids, stream
+_sig("exl2b_qattn_forward_1", c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+     c_void_p, c_void_p, c_int, POINTER(c_uint64), c_int, c_void_p)
+_sig("exl2b_qattn_forward_2", c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(_Chain), POINTER(c_uint64), c_int,
+     c_void_p)
+_sig("exl2b_qmlp_forward", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, POINTER(_Chain), POINTER(c_uint64), c_int,
+     c_void_p)
 _sig("exl2b_gemm_half_q_half_prepared", c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p)
 
 
@@ -115,16 +114,6 @@ class _Lora(Structure):
 
 _sig("exl2b_qattn_set_loras", c_int, c_void_p, POINTER(_Lora), c_int, POINTER(c_int))
 _sig("exl2b_qmlp_set_loras", c_int, c_void_p, POINTER(_Lora), c_int, POINTER(c_int))
-_sig("exl2b_qattn_forward_1_lora", c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-     c_void_p, c_void_p, POINTER(c_uint64), c_int, c_void_p)
-_sig("exl2b_qattn_forward_2_lora", c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(c_uint64), c_int, c_void_p)
-_sig("exl2b_qmlp_forward_lora", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, POINTER(c_uint64), c_int, c_void_p)
-_sig("exl2b_qattn_forward_1_ex_lora", c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-     c_void_p, c_void_p, c_int, POINTER(c_uint64), c_int, c_void_p)
-_sig("exl2b_qattn_forward_2_ex_lora", c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(_Chain), POINTER(c_uint64),
-     c_int, c_void_p)
-_sig("exl2b_qmlp_forward_ex_lora", c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, POINTER(_Chain), POINTER(c_uint64),
-     c_int, c_void_p)
 _sig("exl2b_lora_stack", c_int, POINTER(c_int), c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int),
      POINTER(c_int))
 
@@ -474,22 +463,14 @@ def q_attn_forward_1(q_attn: int, x, batch_size: int, q_len: int, past_len: int,
     accepted and unused (the LoRA launch keeps x·A on chip)."""
     _cuda(x, "x")
     _dtype(x, torch.float16, "x")
-    if loras:
-        ids, n = _lora_ids(loras)
-        _check(lib.exl2b_qattn_forward_1_lora(q_attn, x.data_ptr(), batch_size, q_len, int(past_len), _p(past_lens), q_temp.data_ptr(),
-                                              k_temp.data_ptr(), v_temp.data_ptr(), _p(sin), _p(cos), ids, n, _stream(x)))
-        return
     _check(lib.exl2b_qattn_forward_1(q_attn, x.data_ptr(), batch_size, q_len, int(past_len), _p(past_lens), q_temp.data_ptr(),
-                                     k_temp.data_ptr(), v_temp.data_ptr(), _p(sin), _p(cos), _stream(x)))
+                                     k_temp.data_ptr(), v_temp.data_ptr(), _p(sin), _p(cos), 0, *_lora_ids(loras), _stream(x)))
 
 
 def q_attn_forward_2(q_attn: int, x, attn_output, batch_size: int, q_len: int, loras=(), loras_temp=none_tensor):
     """ext_qattn.cpp:161-191 (loras / loras_temp as q_attn_forward_1)"""
-    if loras:
-        ids, n = _lora_ids(loras)
-        _check(lib.exl2b_qattn_forward_2_lora(q_attn, x.data_ptr(), attn_output.data_ptr(), batch_size, q_len, ids, n, _stream(x)))
-        return
-    _check(lib.exl2b_qattn_forward_2(q_attn, x.data_ptr(), attn_output.data_ptr(), batch_size, q_len, _stream(x)))
+    _check(lib.exl2b_qattn_forward_2(q_attn, x.data_ptr(), attn_output.data_ptr(), batch_size, q_len, 0, None, *_lora_ids(loras),
+                                     _stream(x)))
 
 
 # ---- LoRA (ext_qattn.cpp:194-240, ext_qmlp.cpp q_mlp_set_loras; include/exl2_b200.h "LoRA adapters on the blocks") ----------------
@@ -500,8 +481,9 @@ _lora_keep: dict[int, list] = {}      # handle -> the adapter tensors it points 
 
 
 def _lora_ids(loras):
-    ids = [int(i) for i in loras]
-    return (c_uint64 * len(ids))(*ids), len(ids)
+    """(ids, num_ids) of the block forwards: the active adapter ids as a C array, or (NULL, 0) for none."""
+    ids = [int(i) for i in loras or ()]
+    return ((c_uint64 * len(ids))(*ids) if ids else None), len(ids)
 
 
 def _lora_set(projs) -> tuple:
@@ -613,15 +595,8 @@ def q_mlp_forward_rows(q_mlp: int, x, temp_a, temp_b, loras=(), loras_temp=none_
     _cuda(x, "x")
     _dtype(x, torch.float16, "x")
     rows = x.numel() // x.shape[-1]
-    _mlp_call(q_mlp, x, rows, temp_a.data_ptr(), temp_b.data_ptr(), loras)
-
-
-def _mlp_call(q_mlp: int, x, rows: int, temp_a, temp_b, loras):
-    if loras:
-        ids, n = _lora_ids(loras)
-        _check(lib.exl2b_qmlp_forward_lora(q_mlp, x.data_ptr(), rows, temp_a, temp_b, ids, n, _stream(x)))
-    else:
-        _check(lib.exl2b_qmlp_forward(q_mlp, x.data_ptr(), rows, temp_a, temp_b, _stream(x)))
+    _check(lib.exl2b_qmlp_forward(q_mlp, x.data_ptr(), rows, temp_a.data_ptr(), temp_b.data_ptr(), 0, None, *_lora_ids(loras),
+                                  _stream(x)))
 
 
 def free_q_mlp(handle: int):
@@ -640,7 +615,7 @@ def q_mlp_forward_(q_mlp: int, x, loras=(), loras_temp=none_tensor):
     if rows > temp_a.shape[0]:          # the reference sizes temp_a / temp_b for max_rows at make_q_mlp time and would write past them
         raise RuntimeError(f"q_mlp_forward_: {rows} rows exceed the {temp_a.shape[0]} rows of temp_a given to make_q_mlp "
                            "(use q_mlp_forward_rows with scratch of your own for larger chunks)")
-    _mlp_call(q_mlp, x, rows, temp_a.data_ptr(), _p(temp_b), loras)
+    _check(lib.exl2b_qmlp_forward(q_mlp, x.data_ptr(), rows, temp_a.data_ptr(), _p(temp_b), 0, None, *_lora_ids(loras), _stream(x)))
 
 
 # names the reference's hot-path call sites use (SURVEY.md 8b) that this module provides
@@ -681,37 +656,25 @@ def make_chain(consumers, norm_weight=None) -> "_Chain":
 
 def q_attn_forward_1_ex(q_attn: int, x, batch_size: int, q_len: int, past_len: int, past_lens, q_temp, k_temp, v_temp, sin, cos,
                         input_prepared: bool, loras=()):
-    """loras: active adapter ids (as q_attn_forward_1); a chained call with adapters takes one row (include/exl2_b200.h _ex_lora)"""
-    if loras:
-        ids, n = _lora_ids(loras)
-        _check(lib.exl2b_qattn_forward_1_ex_lora(q_attn, _p(x), batch_size, q_len, int(past_len), _p(past_lens), q_temp.data_ptr(),
-                                                 k_temp.data_ptr(), v_temp.data_ptr(), _p(sin), _p(cos), int(input_prepared), ids, n,
-                                                 _stream(q_temp)))
-        return
-    _check(lib.exl2b_qattn_forward_1_ex(q_attn, _p(x), batch_size, q_len, int(past_len), _p(past_lens), q_temp.data_ptr(),
-                                        k_temp.data_ptr(), v_temp.data_ptr(), _p(sin), _p(cos), int(input_prepared), _stream(q_temp)))
+    """loras: active adapter ids (as q_attn_forward_1); a chained call with adapters takes one row (include/exl2_b200.h
+    "block forwards")"""
+    _check(lib.exl2b_qattn_forward_1(q_attn, _p(x), batch_size, q_len, int(past_len), _p(past_lens), q_temp.data_ptr(),
+                                     k_temp.data_ptr(), v_temp.data_ptr(), _p(sin), _p(cos), int(input_prepared), *_lora_ids(loras),
+                                     _stream(q_temp)))
 
 
 def q_attn_forward_2_ex(q_attn: int, x, attn_output, batch_size: int, q_len: int, input_prepared: bool, chain=None, loras=()):
     ch = ctypes.byref(chain) if chain is not None else None
-    if loras:
-        ids, n = _lora_ids(loras)
-        _check(lib.exl2b_qattn_forward_2_ex_lora(q_attn, x.data_ptr(), _p(attn_output), batch_size, q_len, int(input_prepared), ch,
-                                                 ids, n, _stream(x)))
-        return
-    _check(lib.exl2b_qattn_forward_2_ex(q_attn, x.data_ptr(), _p(attn_output), batch_size, q_len, int(input_prepared), ch, _stream(x)))
+    _check(lib.exl2b_qattn_forward_2(q_attn, x.data_ptr(), _p(attn_output), batch_size, q_len, int(input_prepared), ch,
+                                     *_lora_ids(loras), _stream(x)))
 
 
 def q_mlp_forward_ex(q_mlp: int, x, input_prepared: bool, chain=None, loras=()):
     temp_a, temp_b = _mlp_temps[q_mlp]
     rows = x.numel() // x.shape[-1]
     ch = ctypes.byref(chain) if chain is not None else None
-    if loras:
-        ids, n = _lora_ids(loras)
-        _check(lib.exl2b_qmlp_forward_ex_lora(q_mlp, x.data_ptr(), rows, temp_a.data_ptr(), _p(temp_b), int(input_prepared), ch,
-                                              ids, n, _stream(x)))
-        return
-    _check(lib.exl2b_qmlp_forward_ex(q_mlp, x.data_ptr(), rows, temp_a.data_ptr(), _p(temp_b), int(input_prepared), ch, _stream(x)))
+    _check(lib.exl2b_qmlp_forward(q_mlp, x.data_ptr(), rows, temp_a.data_ptr(), _p(temp_b), int(input_prepared), ch,
+                                  *_lora_ids(loras), _stream(x)))
 
 
 def gemm_half_q_half_prepared(b: int, c, has_norm: bool, norm_eps: float, clear: bool = True):

@@ -344,7 +344,7 @@ class ExLlamaV2Decoder:
         measured slower than the dense path on the 7B preset (DESIGN.md §7), so those steps stay un-chained.  With active
         adapters only one row on the integer GEMV: there each launch leaves its output as a plain row plus a copy for its consumer,
         which forms RMSNorm, RoPE and act·mul itself, so a LoRA launch after it can add the deltas to both (include/exl2_b200.h
-        _ex_lora).  Above one row the chained launches fuse RoPE, act·mul and the RMSNorm sums into their epilogues, where no
+        "block forwards").  Above one row the chained launches fuse RoPE, act·mul and the RMSNorm sums into their epilogues, where no
         delta can be added after them, so adapted steps stay on the un-chained block forms."""
         wide = q_len == 1 and GEMM_BIG_MIN_ROWS < rows <= DECODE_CHAIN_ROWS
         if not (self.chained and self.fused_attn and (rows <= 8 or wide)):

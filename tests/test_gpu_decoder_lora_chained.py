@@ -1,4 +1,4 @@
-"""Batch-1 decode with LoRA adapters on the chained step (include/exl2_b200.h _ex_lora, csrc/lora.cu's one-row form).
+"""Batch-1 decode with LoRA adapters on the chained step (include/exl2_b200.h "block forwards", csrc/lora.cu's one-row form).
 
 - Zero-B adapters (B = 0) on all seven projections leave the chained step's logits byte-identical to the adapter-free chained
   step's, eager and graph-replayed, on the 7B preset and test-small: a wrong mirror index or an ordering hazard between a LoRA
